@@ -84,6 +84,12 @@ def _declare(lib):
         "ark_arrow_to_json_create": (C.c_int, [C.c_char_p, P(vp)]),
         "ark_arrow_to_json_process": (C.c_int, [vp, P(ArrowArray), P(ArrowSchema), P(ArrowArray), P(ArrowSchema)]),
         "ark_arrow_to_json_process_device": (C.c_int, [vp, P(ArrowDeviceArray), P(ArrowSchema), P(ArrowDeviceArray), P(ArrowSchema)]),
+        "ark_protobuf_to_arrow_create": (C.c_int, [C.c_char_p, P(vp)]),
+        "ark_protobuf_to_arrow_process": (C.c_int, [vp, P(ArrowArray), P(ArrowSchema), P(ArrowArray), P(ArrowSchema)]),
+        "ark_protobuf_to_arrow_process_device": (C.c_int, [vp, P(ArrowDeviceArray), P(ArrowSchema), P(ArrowDeviceArray), P(ArrowSchema)]),
+        "ark_arrow_to_protobuf_create": (C.c_int, [C.c_char_p, P(vp)]),
+        "ark_arrow_to_protobuf_process": (C.c_int, [vp, P(ArrowArray), P(ArrowSchema), P(ArrowArray), P(ArrowSchema)]),
+        "ark_arrow_to_protobuf_process_device": (C.c_int, [vp, P(ArrowDeviceArray), P(ArrowSchema), P(ArrowDeviceArray), P(ArrowSchema)]),
         "ark_expr_evaluate": (C.c_int, [C.c_char_p, P(ArrowArray), P(ArrowSchema), P(ArrowArray), P(ArrowSchema), P(C.c_int)]),
         "ark_expr_evaluate_device": (C.c_int, [C.c_char_p, P(ArrowDeviceArray), P(ArrowSchema), P(ArrowDeviceArray), P(ArrowSchema), P(C.c_int)]),
         "ark_proc_close": (C.c_int, [vp]),

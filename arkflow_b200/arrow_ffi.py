@@ -45,8 +45,14 @@ def release_array(arr: L.ArrowArray):
 # device
 # ---------------------------------------------------------------------------------------------
 
-_FMT = {"int64": b"l", "float64": b"g", "utf8": b"u", "binary": b"z", "bool": b"b", "null": b"n"}
+_FMT = {"int64": b"l", "float64": b"g", "utf8": b"u", "binary": b"z", "bool": b"b", "null": b"n",
+        "int32": b"i", "uint32": b"I", "uint64": b"L", "float32": b"f"}
 _FMT_INV = {v: k for k, v in _FMT.items()}
+# fixed-width column types: (array-interface / numpy typestr, bytes per value, torch dtype name, pyarrow type factory).
+# int32 / uint32 / uint64 / float32 columns come from protobuf_to_arrow and feed arrow_to_protobuf.
+_FIXED = {"int64": ("<i8", 8, "int64", pa.int64), "float64": ("<f8", 8, "float64", pa.float64),
+          "int32": ("<i4", 4, "int32", pa.int32), "uint32": ("<u4", 4, "uint32", pa.uint32),
+          "uint64": ("<u8", 8, "uint64", pa.uint64), "float32": ("<f4", 4, "float32", pa.float32)}
 
 
 class DeviceColumn:
@@ -266,8 +272,9 @@ class DeviceBatch:
                 continue
             validity = view(0, (n + 7) // 8, "|u1", 1, torch.uint8) if (a.n_buffers > 0 and a.buffers[0]) else None
             offsets = None
-            if dtype in ("int64", "float64"):
-                data = view(1, n * 8, "<i8" if dtype == "int64" else "<f8", 8, torch.int64 if dtype == "int64" else torch.float64)
+            if dtype in _FIXED:
+                ts, w, tname, _ = _FIXED[dtype]
+                data = view(1, n * w, ts, w, getattr(torch, tname))
             elif dtype == "bool":
                 data = view(1, (n + 7) // 8, "|u1", 1, torch.uint8)
             else:
@@ -289,8 +296,8 @@ class DeviceBatch:
                 arrays.append(pa.nulls(n))
                 fields.append(pa.field(c.name, pa.null(), nullable=True))
                 continue
-            if c.dtype in ("int64", "float64"):
-                t = pa.int64() if c.dtype == "int64" else pa.float64()
+            if c.dtype in _FIXED:
+                t = _FIXED[c.dtype][3]()
                 arr = pa.Array.from_buffers(t, n, [vbuf, pa.py_buffer(c.data.cpu().numpy().tobytes())], null_count=nulls)
             elif c.dtype == "bool":
                 arr = pa.Array.from_buffers(pa.bool_(), n, [vbuf, pa.py_buffer(c.data.cpu().numpy().tobytes())], null_count=nulls)
@@ -325,9 +332,10 @@ class DeviceBatch:
             bufs = arr.buffers()
             n = len(arr)
             validity = up(bufs[0], np.uint8) if (bufs[0] is not None and arr.null_count) else None
-            if pa.types.is_int64(arr.type) or pa.types.is_float64(arr.type):
-                dt = "int64" if pa.types.is_int64(arr.type) else "float64"
-                data = up(bufs[1], np.int64 if dt == "int64" else np.float64, n)
+            fixed = [k for k, v in _FIXED.items() if arr.type == v[3]()]
+            if fixed:
+                dt = fixed[0]
+                data = up(bufs[1], np.dtype(_FIXED[dt][0]), n)
                 cols.append(DeviceColumn(name, dt, n, data, None, validity, arr.null_count, f.nullable))
             elif pa.types.is_boolean(arr.type):
                 cols.append(DeviceColumn(name, "bool", n, up(bufs[1], np.uint8), None, validity, arr.null_count, f.nullable))

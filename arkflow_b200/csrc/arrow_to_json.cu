@@ -278,6 +278,11 @@ std::string json_escape_key(const std::string& name) {
 
 }  // namespace
 
+// zero-column batch → zero lines → length mismatch in new_binary_with_origin
+void fail_filtered_to_no_columns() {
+  fail(ARK_ERR_PROCESS, "Creating an Arrow record batch failed: Invalid argument error: all columns in a record batch must have the same length");
+}
+
 struct ArrowToJsonProcessor : Processor {
   const char* type() const override { return "arrow_to_json"; }
   bool has_include = false;
@@ -321,8 +326,7 @@ Batch arrow_to_json_device(const Processor& proc, Batch& in, cudaStream_t stream
     memcpy(a.key, key.data(), key.size());
     a.view = c.view();
   }
-  if (ap.has_include && P.n_cols == 0 && n > 0)  // zero-column batch → zero lines → length mismatch in new_binary_with_origin
-    fail(ARK_ERR_PROCESS, "Creating an Arrow record batch failed: Invalid argument error: all columns in a record batch must have the same length");
+  if (ap.has_include && P.n_cols == 0 && n > 0) fail_filtered_to_no_columns();
   BufferPtr lens = device_alloc((size_t)(n + 1) * 4), offs = device_alloc((size_t)(n + 1) * 4);
   ARK_CUDA(cudaMemsetAsync(lens.get(), 0, (size_t)(n + 1) * 4, stream));
   const unsigned grid = (unsigned)std::max<int64_t>(1, ceil_div(n, 128));

@@ -313,6 +313,15 @@ static bool format_supported(const std::string& f) {
   return f == "l" || f == "g" || f == "u" || f == "z" || f == "b";
 }
 
+// the fixed-width types only the protobuf codec reads (import_*'s codec_types)
+static DType codec_dtype(const std::string& f) {
+  if (f == "i") return DType::Int32;
+  if (f == "I") return DType::UInt32;
+  if (f == "L") return DType::UInt64;
+  if (f == "f") return DType::Float32;
+  return DType::Null;
+}
+
 // ---- import ---------------------------------------------------------------------------------------------
 // Host → device copy of one Arrow buffer.  A Rust shim hands over arrow-rs heap buffers, i.e. PAGEABLE memory: a plain
 // cudaMemcpyAsync from such a pointer is staged by the driver through one small pinned buffer, synchronously, at a
@@ -466,7 +475,7 @@ static void h2d(void* dst, const void* src, size_t n, cudaStream_t s, int64_t* a
 }
 
 Batch import_host(const ArrowArray* arr, const ArrowSchema* schema, const std::vector<bool>* needed,
-                  cudaStream_t stream, int64_t* h2d_bytes) {
+                  cudaStream_t stream, int64_t* h2d_bytes, bool codec_types) {
   std::vector<Field> fields = schema_fields(schema);
   if (arr->n_children != (int64_t)fields.size())
     fail(ARK_ERR_PROCESS, "Registration failed: array/schema child count mismatch");
@@ -476,9 +485,10 @@ Batch import_host(const ArrowArray* arr, const ArrowSchema* schema, const std::v
   for (size_t i = 0; i < fields.size(); ++i) {
     Column c;
     c.field = fields[i];
+    if (codec_types && codec_dtype(c.field.format) != DType::Null) c.field.type = codec_dtype(c.field.format);
     const ArrowArray* a = arr->children[i];
     c.length = a->length;
-    bool want = (!needed || (*needed)[i]) && format_supported(fields[i].format);
+    bool want = (!needed || (*needed)[i]) && (format_supported(fields[i].format) || c.field.type != fields[i].type);
     if (!want) { c.present = false; b.cols.push_back(std::move(c)); continue; }
     if (a->length != arr->length) fail(ARK_ERR_PROCESS, "Registration failed: column length mismatch");
     int64_t off = a->offset, n = a->length;
@@ -495,11 +505,12 @@ Batch import_host(const ArrowArray* arr, const ArrowSchema* schema, const std::v
       c.null_count = 0;
     }
     switch (c.field.type) {
-      case DType::Int64:
-      case DType::Float64: {
-        BufferPtr d = device_alloc((size_t)n * 8);
-        if (n) h2d(d.get(), (const uint8_t*)a->buffers[1] + off * 8, (size_t)n * 8, stream, h2d_bytes);
-        c.data = (const uint8_t*)d.get(); c.data_bytes = n * 8; c.owners.push_back(d);
+      case DType::Int64: case DType::Float64:
+      case DType::Int32: case DType::UInt32: case DType::UInt64: case DType::Float32: {
+        const int w = fixed_width(c.field.type);
+        BufferPtr d = device_alloc((size_t)n * w);
+        if (n) h2d(d.get(), (const uint8_t*)a->buffers[1] + off * w, (size_t)n * w, stream, h2d_bytes);
+        c.data = (const uint8_t*)d.get(); c.data_bytes = n * w; c.owners.push_back(d);
         break;
       }
       case DType::Bool: {
@@ -542,7 +553,7 @@ __global__ void gather_extents_kernel(const int32_t* const* offs, const int64_t*
 }
 
 Batch import_device(const ArrowDeviceArray* darr, const ArrowSchema* schema, const std::vector<bool>* needed,
-                    BufferPtr keep) {
+                    BufferPtr keep, bool codec_types) {
   if (darr->device_type != ARROW_DEVICE_CUDA && darr->device_type != ARROW_DEVICE_CUDA_HOST)
     fail(ARK_ERR_PROCESS, "Registration failed: ArrowDeviceArray is not on a CUDA device");
   const ArrowArray* arr = &darr->array;
@@ -557,9 +568,10 @@ Batch import_device(const ArrowDeviceArray* darr, const ArrowSchema* schema, con
   for (size_t i = 0; i < fields.size(); ++i) {
     Column c;
     c.field = fields[i];
+    if (codec_types && codec_dtype(c.field.format) != DType::Null) c.field.type = codec_dtype(c.field.format);
     const ArrowArray* a = arr->children[i];
     c.length = a->length;
-    bool want = (!needed || (*needed)[i]) && format_supported(fields[i].format);
+    bool want = (!needed || (*needed)[i]) && (format_supported(fields[i].format) || c.field.type != fields[i].type);
     if (!want) { c.present = false; b.cols.push_back(std::move(c)); continue; }
     if (a->length != arr->length) fail(ARK_ERR_PROCESS, "Registration failed: column length mismatch");
     int64_t off = a->offset, n = a->length;
@@ -571,7 +583,10 @@ Batch import_device(const ArrowDeviceArray* darr, const ArrowSchema* schema, con
     } else c.null_count = 0;
     switch (c.field.type) {
       case DType::Int64: case DType::Float64:
-        c.data = (const uint8_t*)a->buffers[1] + off * 8; c.data_bytes = n * 8; break;
+      case DType::Int32: case DType::UInt32: case DType::UInt64: case DType::Float32: {
+        const int w = fixed_width(c.field.type);
+        c.data = (const uint8_t*)a->buffers[1] + off * w; c.data_bytes = n * w; break;
+      }
       case DType::Bool:
         c.data = (const uint8_t*)a->buffers[1] + (off >> 3); c.data_bit0 = (int32_t)(off & 7);
         c.data_bytes = (n + 7) / 8 + 1; break;
@@ -785,7 +800,8 @@ static ExportCol normalise_for_export(const Column& c_in, bool to_host, cudaStre
   }
   switch (c.field.type) {
     case DType::Int64: case DType::Float64:
-      e.buf1 = c.data; e.buf1_bytes = n * 8; e.n_buffers = 2; break;
+    case DType::Int32: case DType::UInt32: case DType::UInt64: case DType::Float32:
+      e.buf1 = c.data; e.buf1_bytes = n * fixed_width(c.field.type); e.n_buffers = 2; break;
     case DType::Bool:
       e.buf1_bytes = (n + 7) / 8;
       if (c.data_bit0 != 0 && n > 0) {

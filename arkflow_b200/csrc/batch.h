@@ -125,15 +125,25 @@ struct Batch {
 std::vector<Field> schema_fields(const ArrowSchema* s);  // struct schema → fields (no data needed)
 std::string schema_fingerprint(const std::vector<Field>& f);
 
+// Bytes per value of a fixed-width column type other than Boolean; 0 for the rest.
+inline int fixed_width(DType t) {
+  switch (t) {
+    case DType::Int64: case DType::Float64: case DType::UInt64: return 8;
+    case DType::Int32: case DType::UInt32: case DType::Float32: return 4;
+    default: return 0;
+  }
+}
+
 // Import a struct array.  `needed`: per top-level column, whether its buffers are required (others
 // get present=false and are not copied); nullptr ⇒ all.  Host import copies buffers to HBM on
 // `stream` (the source is read asynchronously when pinned; the caller synchronizes before
 // releasing `arr`).  Device import wraps the pointers without copying; `keep` (may be null) is
-// attached to every column as an owner.
+// attached to every column as an owner.  `codec_types` also imports Int32 / UInt32 / UInt64 / Float32
+// columns (formats i, I, L, f): only arrow_to_protobuf reads them; every other caller leaves them not present.
 Batch import_host(const ArrowArray* arr, const ArrowSchema* schema, const std::vector<bool>* needed,
-                  cudaStream_t stream, int64_t* h2d_bytes = nullptr);
+                  cudaStream_t stream, int64_t* h2d_bytes = nullptr, bool codec_types = false);
 Batch import_device(const ArrowDeviceArray* arr, const ArrowSchema* schema, const std::vector<bool>* needed,
-                    BufferPtr keep);
+                    BufferPtr keep, bool codec_types = false);
 
 // Export: builds a struct ArrowArray/ArrowSchema whose release callbacks drop the owners.
 // Host export copies HBM → pinned host on `stream` and synchronizes it.

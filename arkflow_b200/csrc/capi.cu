@@ -346,6 +346,100 @@ int ark_arrow_to_json_process_device(ark_proc_t* p, ArrowDeviceArray* in, ArrowS
   });
 }
 
+// ---- protobuf_to_arrow / arrow_to_protobuf (processor/protobuf.rs:98-148) --------------------------------------
+static int create_proc(std::unique_ptr<Processor> (*make)(const char*), const char* config_json, ark_proc_t** out) {
+  return guarded([&] {
+    if (!out) fail(ARK_ERR_PROCESS, "null output handle");
+    *out = nullptr;
+    auto p = make(config_json);
+    auto* h = new ark_proc();
+    h->impl = std::move(p);
+    *out = h;
+  });
+}
+
+static Processor* as_type(ark_proc_t* p, const char* type) {
+  if (!p || !p->impl || strcmp(p->impl->type(), type) != 0) fail(ARK_ERR_PROCESS, std::string("handle is not a ") + type + " processor");
+  return p->impl.get();
+}
+
+int ark_protobuf_to_arrow_create(const char* config_json, ark_proc_t** out) { return create_proc(make_protobuf_to_arrow, config_json, out); }
+
+static std::vector<bool> protobuf_mask(const Processor& pp, const std::vector<Field>& fields) {
+  std::vector<bool> m(fields.size(), false);
+  for (size_t i = 0; i < fields.size(); ++i) if (fields[i].name == protobuf_to_arrow_value_field(pp)) m[i] = true;
+  return m;
+}
+
+int ark_protobuf_to_arrow_process(ark_proc_t* p, ArrowArray* in, ArrowSchema* in_schema, ArrowArray* out, ArrowSchema* out_schema) {
+  BufferPtr in_owner = adopt_array(in);
+  return guarded([&] {
+    Processor* pp = as_type(p, "protobuf_to_arrow");
+    const ArrowArray* arr = (const ArrowArray*)in_owner.get();
+    if (!arr) fail(ARK_ERR_PROCESS, "input array already released");
+    if (arr->length == 0) { set_none(out, out_schema); return; }  // ProcessResult::None, protobuf.rs:101-103
+    std::vector<Field> fields = schema_fields(in_schema);
+    std::vector<bool> mask = protobuf_mask(*pp, fields);
+    StreamLease lease;
+    Batch b = import_host(arr, in_schema, &mask, lease.s);
+    Batch r = protobuf_to_arrow_device(*pp, b, lease.s);
+    export_host(r, lease.s, out, out_schema);
+  });
+}
+
+int ark_protobuf_to_arrow_process_device(ark_proc_t* p, ArrowDeviceArray* in, ArrowSchema* in_schema, ArrowDeviceArray* out,
+                                         ArrowSchema* out_schema) {
+  BufferPtr in_owner = adopt_array(&in->array);
+  return guarded([&] {
+    Processor* pp = as_type(p, "protobuf_to_arrow");
+    if (!in_owner) fail(ARK_ERR_PROCESS, "input array already released");
+    ArrowDeviceArray view = *in;
+    view.array = *(const ArrowArray*)in_owner.get();
+    if (view.array.length == 0) { memset(out, 0, sizeof(*out)); if (out_schema) memset(out_schema, 0, sizeof(*out_schema)); return; }
+    std::vector<Field> fields = schema_fields(in_schema);
+    std::vector<bool> mask = protobuf_mask(*pp, fields);
+    StreamLease lease;
+    Batch b = import_device(&view, in_schema, &mask, in_owner);
+    Batch r = protobuf_to_arrow_device(*pp, b, lease.s);
+    export_device(r, out, out_schema);
+  });
+}
+
+int ark_arrow_to_protobuf_create(const char* config_json, ark_proc_t** out) { return create_proc(make_arrow_to_protobuf, config_json, out); }
+
+int ark_arrow_to_protobuf_process(ark_proc_t* p, ArrowArray* in, ArrowSchema* in_schema, ArrowArray* out, ArrowSchema* out_schema) {
+  BufferPtr in_owner = adopt_array(in);
+  return guarded([&] {
+    Processor* pp = as_type(p, "arrow_to_protobuf");
+    const ArrowArray* arr = (const ArrowArray*)in_owner.get();
+    if (!arr) fail(ARK_ERR_PROCESS, "input array already released");
+    if (arr->length == 0) { set_none(out, out_schema); return; }  // ProcessResult::None, protobuf.rs:101-103
+    StreamLease lease;
+    Batch b = import_host(arr, in_schema, nullptr, lease.s, nullptr, true);
+    Batch r = arrow_to_protobuf_device(*pp, b, lease.s);
+    export_host(r, lease.s, out, out_schema);
+  });
+}
+
+int ark_arrow_to_protobuf_process_device(ark_proc_t* p, ArrowDeviceArray* in, ArrowSchema* in_schema, ArrowDeviceArray* out,
+                                         ArrowSchema* out_schema) {
+  BufferPtr in_owner = adopt_array(&in->array);
+  return guarded([&] {
+    Processor* pp = as_type(p, "arrow_to_protobuf");
+    if (!in_owner) fail(ARK_ERR_PROCESS, "input array already released");
+    ArrowDeviceArray view = *in;
+    view.array = *(const ArrowArray*)in_owner.get();
+    if (view.array.length == 0) { memset(out, 0, sizeof(*out)); if (out_schema) memset(out_schema, 0, sizeof(*out_schema)); return; }
+    StreamLease lease;
+    Batch b = import_device(&view, in_schema, nullptr, in_owner, true);
+    std::vector<Column*> all;
+    for (auto& c : b.cols) all.push_back(&c);
+    resolve_varlen_extents_many(all, lease.s);
+    Batch r = arrow_to_protobuf_device(*pp, b, lease.s);
+    export_device(r, out, out_schema);
+  });
+}
+
 // ---- expr::evaluate_expr (plugin/expr/mod.rs:92-122) ---------------------------------------------------
 namespace {
 

@@ -1,6 +1,7 @@
 // engine.h — host-side processors: the C++ mirror of the reference's plugin objects for this path.
 //   SqlProcessor        ← crates/arkflow-plugin/src/processor/sql.rs:59-225
 //   JsonToArrow / ArrowToJson ← crates/arkflow-plugin/src/processor/json.rs:42-113
+//   ProtobufToArrow / ArrowToProtobuf ← crates/arkflow-plugin/src/processor/protobuf.rs:33-244
 #pragma once
 #include <map>
 #include <memory>
@@ -80,6 +81,13 @@ struct TakeSpec { const Column* src; int side; std::string name; bool may_miss; 
 std::vector<Column> take_columns(const std::vector<TakeSpec>& specs, const unsigned int* idx0, const unsigned int* idx1, int64_t n, cudaStream_t stream);
 std::unique_ptr<Processor> make_arrow_to_json(const char* config_json);
 Batch arrow_to_json_device(const Processor& proc, Batch& in, cudaStream_t stream);
+// `fields_to_include` kept none of a non-empty batch's columns (arrow_to_json, arrow_to_protobuf)
+[[noreturn]] void fail_filtered_to_no_columns();
+std::unique_ptr<Processor> make_protobuf_to_arrow(const char* config_json);
+const std::string& protobuf_to_arrow_value_field(const Processor& p);
+Batch protobuf_to_arrow_device(const Processor& proc, Batch& in, cudaStream_t stream);
+std::unique_ptr<Processor> make_arrow_to_protobuf(const char* config_json);
+Batch arrow_to_protobuf_device(const Processor& proc, Batch& in, cudaStream_t stream);
 Batch concat_device(std::vector<Batch>& ins, cudaStream_t stream);
 Batch synth_batch(int64_t n, int64_t row0, uint64_t seed, int value_kind, int64_t key_space, cudaStream_t stream);
 

@@ -11,6 +11,7 @@
 // every output byte written once (SURVEY.md §8(d): 36 B/row for config 2).
 #include "batch.h"
 #include "filter_project.cuh"
+#include "utf8.cuh"
 #include "vm.cuh"
 
 namespace ark {
@@ -347,35 +348,12 @@ __global__ void pack_bits_kernel(const uint8_t* bytes, int64_t n, uint8_t* bitma
   if ((threadIdx.x & 31) == 0 && z && zeros) atomicAdd(zeros, (unsigned long long)z);
 }
 
-// One thread validates one string (well-formed UTF-8 per Unicode table 3-7: no overlongs, no
-// surrogates, ≤ U+10FFFF).  Raises *bad when any non-NULL string is invalid.
+// One thread validates one string (utf8_valid).  Raises *bad when any non-NULL string is invalid.
 __global__ void utf8_validate_kernel(const int32_t* offsets, const uint8_t* data, const uint8_t* validity, int vbit0, long long n, int* bad) {
   const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= n) return;
   if (validity && !((validity[(r + vbit0) >> 3] >> ((r + vbit0) & 7)) & 1)) return;
-  const uint8_t* p = data + offsets[r];
-  const int len = offsets[r + 1] - offsets[r];
-  int i = 0;
-  bool ok = true;
-  while (i < len) {
-    const uint8_t b0 = p[i];
-    if (b0 < 0x80) { ++i; continue; }
-    int need; uint8_t lo = 0x80, hi = 0xBF;
-    if (b0 >= 0xC2 && b0 <= 0xDF) need = 1;
-    else if (b0 == 0xE0) { need = 2; lo = 0xA0; }
-    else if ((b0 >= 0xE1 && b0 <= 0xEC) || b0 == 0xEE || b0 == 0xEF) need = 2;
-    else if (b0 == 0xED) { need = 2; hi = 0x9F; }
-    else if (b0 == 0xF0) { need = 3; lo = 0x90; }
-    else if (b0 >= 0xF1 && b0 <= 0xF3) need = 3;
-    else if (b0 == 0xF4) { need = 3; hi = 0x8F; }
-    else { ok = false; break; }
-    if (i + need >= len) { ok = false; break; }  // truncated sequence
-    if (p[i + 1] < lo || p[i + 1] > hi) { ok = false; break; }
-    for (int k = 2; k <= need; ++k) if ((p[i + k] & 0xC0) != 0x80) { ok = false; break; }
-    if (!ok) break;
-    i += need + 1;
-  }
-  if (!ok) atomicExch(bad, 1);
+  if (!utf8_valid(data + offsets[r], offsets[r + 1] - offsets[r])) atomicExch(bad, 1);
 }
 
 template <int PRED, int NV>

@@ -12,8 +12,10 @@
 
 namespace ark {
 
-// List / Struct: columns this library produces itself (json_to_arrow of nested values); never query operands
-enum class DType : uint8_t { Null = 0, Bool = 1, Int64 = 2, Float64 = 3, Utf8 = 4, Binary = 5, List = 6, Struct = 7 };
+// List / Struct: columns this library produces itself (json_to_arrow of nested values); never query operands.
+// Int32 / UInt32 / UInt64 / Float32: only the protobuf codec produces and reads them (protobuf.cu); never query operands.
+enum class DType : uint8_t { Null = 0, Bool = 1, Int64 = 2, Float64 = 3, Utf8 = 4, Binary = 5, List = 6, Struct = 7,
+                             Int32 = 8, UInt32 = 9, UInt64 = 10, Float32 = 11 };
 const char* dtype_name(DType t);         // DataFusion display name: Int64, Float64, Utf8, …
 const char* dtype_arrow_format(DType t); // Arrow C format string: "l", "g", "u", "z", "b", "n"
 

@@ -25,6 +25,10 @@ const char* dtype_name(DType t) {
     case DType::Binary: return "Binary";
     case DType::List: return "List";
     case DType::Struct: return "Struct";
+    case DType::Int32: return "Int32";
+    case DType::UInt32: return "UInt32";
+    case DType::UInt64: return "UInt64";
+    case DType::Float32: return "Float32";
   }
   return "?";
 }
@@ -38,6 +42,10 @@ const char* dtype_arrow_format(DType t) {
     case DType::Binary: return "z";
     case DType::List: return "+l";
     case DType::Struct: return "+s";
+    case DType::Int32: return "i";
+    case DType::UInt32: return "I";
+    case DType::UInt64: return "L";
+    case DType::Float32: return "f";
   }
   return "n";
 }

@@ -1,7 +1,7 @@
 """Host-side mirror of the reference's Processor plugin surface for the hot path.
 
 Same names, configuration keys and error behaviour as the reference so that the parity tests read
-like the reference's own (crates/arkflow-plugin/src/processor/sql.rs:250-426, json.rs:160-343):
+like the reference's own (crates/arkflow-plugin/src/processor/sql.rs:250-426, json.rs:160-343, protobuf.rs:246-468):
 
     trait Processor        → class Processor            (core/processor/mod.rs:32-79)
     ProcessResult          → class ProcessResult        (core/lib.rs:179-187)
@@ -304,6 +304,43 @@ class ArrowToJsonProcessor(_NativeProcessor):
         super().__init__(config)
 
 
+class _ProtobufProcessor(_NativeProcessor):
+    def __init__(self, config: Optional[dict]):
+        if isinstance(config, dict) and isinstance(config.get("fields_to_include"), (set, frozenset)):
+            config = dict(config, fields_to_include=sorted(config["fields_to_include"]))
+        super().__init__(config)
+
+    def process(self, msg_batch) -> ProcessResult:
+        # both directions build their output with MessageBatch::new_arrow: the input name is not carried over
+        r = super().process(msg_batch)
+        for b in r.batches:
+            if isinstance(b, MessageBatch):
+                b.input_name = None
+        return r
+
+
+class ProtobufToArrowProcessor(_ProtobufProcessor):
+    """`type: protobuf_to_arrow` — crates/arkflow-plugin/src/processor/protobuf.rs:118-139, 197-214.
+
+    config (flat): {"proto_inputs": [dir, ...], "proto_includes": [dir, ...]?, "message_type": "pkg.Msg",
+    "value_field": "__value__"?}
+    """
+
+    _create, _process, _process_device = ("ark_protobuf_to_arrow_create", "ark_protobuf_to_arrow_process",
+                                          "ark_protobuf_to_arrow_process_device")
+
+
+class ArrowToProtobufProcessor(_ProtobufProcessor):
+    """`type: arrow_to_protobuf` — crates/arkflow-plugin/src/processor/protobuf.rs:106-117, 215-232.
+
+    config (flat): {"proto_inputs": [dir, ...], "proto_includes": [dir, ...]?, "message_type": "pkg.Msg",
+    "fields_to_include": [name, ...]?}
+    """
+
+    _create, _process, _process_device = ("ark_arrow_to_protobuf_create", "ark_arrow_to_protobuf_process",
+                                          "ark_arrow_to_protobuf_process_device")
+
+
 class BatchProcessor(Processor):
     """`type: batch` {count, timeout_ms} — processor/batch.rs:37-124.  Holds the incoming batches in HBM and
     returns their concatenation once `count` of them are held or `timeout_ms` has passed since the last flush."""
@@ -375,6 +412,7 @@ def build_processor(config: dict) -> Processor:
 def init() -> None:
     """plugin::processor::init for the hot-path processors (processor/mod.rs:28-35)."""
     for t, cls in (("sql", SqlProcessor), ("json_to_arrow", JsonToArrowProcessor), ("arrow_to_json", ArrowToJsonProcessor),
+                   ("protobuf_to_arrow", ProtobufToArrowProcessor), ("arrow_to_protobuf", ArrowToProtobufProcessor),
                    ("batch", BatchProcessor)):
         if t not in _PROCESSOR_BUILDERS:
             register_processor_builder(t, lambda name, cfg, _c=cls: _c(cfg))

@@ -91,7 +91,7 @@ typedef enum ark_status {
   ARK_ERR_EOF = 6          /* Error::EOF (buffer closed and drained)                                 */
 } ark_status;
 
-typedef struct ark_proc ark_proc_t; /* a built Processor (sql / json_to_arrow / arrow_to_json)       */
+typedef struct ark_proc ark_proc_t; /* a built Processor (sql / json_to_arrow / arrow_to_json / protobuf_to_arrow / arrow_to_protobuf) */
 typedef struct ark_buf ark_buf_t;   /* a built Buffer (memory / session_window / tumbling_window / sliding_window) */
 typedef struct ark_batcher ark_batcher_t; /* a built `batch` processor                                  */
 typedef struct ark_dist ark_dist_t; /* one rank's end of the device-side GROUP BY exchange              */
@@ -145,6 +145,41 @@ int ark_arrow_to_json_process(ark_proc_t* p, struct ArrowArray* in, struct Arrow
 int ark_arrow_to_json_process_device(ark_proc_t* p, struct ArrowDeviceArray* in,
                                      struct ArrowSchema* in_schema, struct ArrowDeviceArray* out,
                                      struct ArrowSchema* out_schema);
+
+/* ---- `protobuf_to_arrow` / `arrow_to_protobuf` processors: replace {ProtobufToArrow,ArrowToProtobuf}
+ *      ProcessorBuilder::build, ProtobufProcessor::{new,process} and the conversions they call,
+ *      crates/arkflow-plugin/src/processor/protobuf.rs:197-232, 71-148 and
+ *      crates/arkflow-plugin/src/component/protobuf.rs:41-339 ---- */
+/* config_json: {"proto_inputs": ["dir", …], "proto_includes": ["dir", …]?, "message_type": "pkg.Msg",
+ * "value_field": "__value__"? (protobuf_to_arrow), "fields_to_include": ["a", …]? (arrow_to_protobuf)}.
+ * Deliberate deviation: the keys are read flat, the shape the reference's documentation
+ * (docs/docs/components/2-processors/protobuf.md) and examples/protobuf_example.yaml use; the reference's
+ * ArrowToProtobufProcessorConfig nests them under `c` (protobuf.rs:165-169, no #[serde(flatten)]) and so
+ * rejects its own documented shape with "missing field `c`".
+ * Every `*.proto` file directly inside each proto_inputs directory is parsed (imports resolved against
+ * proto_includes, default proto_inputs) on the host, without a CUDA device.  NULL config → ARK_ERR_CONFIG
+ * ("ProtobufToArrow processor configuration is missing" / "ArrowToProtobuf …"); a missing or mistyped key →
+ * ARK_ERR_SERIALIZATION; no .proto file → ARK_ERR_CONFIG ("No proto files found in the specified paths…");
+ * a parse or type-resolution error → ARK_ERR_CONFIG ("Failed to parse the proto file: …"); an unknown
+ * message → ARK_ERR_CONFIG ("The message type could not be found: <name>").
+ * An empty batch gives no output (ProcessResult::None, protobuf.rs:101-103); a batch of only NULL payloads gives zero
+ * rows with the message's columns (the reference panics there).  Library limits, not reference behaviour:
+ * protobuf_to_arrow of a message with more than 64 fields, and arrow_to_protobuf encoding more than 64 fields, return
+ * ARK_ERR_UNSUPPORTED; an output string / binary column of 2 GiB or more returns ARK_ERR_PROCESS.  protobuf_to_arrow decodes the
+ * Binary column `value_field` into one non-nullable column per message field; arrow_to_protobuf appends a
+ * non-null Binary `__value__` column to the input.  Error rules: csrc/protobuf.cu. */
+int ark_protobuf_to_arrow_create(const char* config_json, ark_proc_t** out);
+int ark_protobuf_to_arrow_process(ark_proc_t* p, struct ArrowArray* in, struct ArrowSchema* in_schema,
+                                  struct ArrowArray* out, struct ArrowSchema* out_schema);
+int ark_protobuf_to_arrow_process_device(ark_proc_t* p, struct ArrowDeviceArray* in,
+                                         struct ArrowSchema* in_schema, struct ArrowDeviceArray* out,
+                                         struct ArrowSchema* out_schema);
+int ark_arrow_to_protobuf_create(const char* config_json, ark_proc_t** out);
+int ark_arrow_to_protobuf_process(ark_proc_t* p, struct ArrowArray* in, struct ArrowSchema* in_schema,
+                                  struct ArrowArray* out, struct ArrowSchema* out_schema);
+int ark_arrow_to_protobuf_process_device(ark_proc_t* p, struct ArrowDeviceArray* in,
+                                         struct ArrowSchema* in_schema, struct ArrowDeviceArray* out,
+                                         struct ArrowSchema* out_schema);
 
 /* ---- expr::evaluate_expr: replaces crates/arkflow-plugin/src/expr/mod.rs:92-122 (the key expression
  *      of a `temporary_list` entry, processor/sql.rs:151-186) ---- */

@@ -7,6 +7,7 @@ this script feeds DESIGN.md.
   config 4  hash join probe 2^24 x build K unique keys   inputs + output     join_probe_kernel (+ gathers)
   config 5  window concat of k batches                   2 x bytes           concat_copy_kernel
   json      json_to_arrow of 63-byte messages            67 B in + 26 B out  json_parse_kernel
+  protobuf  arrow_to_protobuf + protobuf_to_arrow of 2^22 schema-S rows, and the JSON pair on the same rows
 
 Usage: python scripts/bench_configs.py [--rows 16777216] [--reps 5] [--out configs.json]
 """
@@ -27,7 +28,7 @@ def main():
     ap.add_argument("--keys", type=int, default=1_000_000)
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--out", default="")
-    ap.add_argument("--only", default="", help="comma-separated legs: groupby,join,concat,json (default: all)")
+    ap.add_argument("--only", default="", help="comma-separated legs: groupby,join,concat,json,tojson,protobuf (default: all)")
     args = ap.parse_args()
 
     import numpy as np
@@ -75,7 +76,7 @@ def main():
 
     results = {"peak_gbs": peak, "rows": args.rows, "keys": args.keys}
     n = args.rows
-    legs = set(args.only.split(",")) if args.only else {"groupby", "join", "concat", "json", "tojson"}
+    legs = set(args.only.split(",")) if args.only else {"groupby", "join", "concat", "json", "tojson", "protobuf"}
 
     # ---- config 3: GROUP BY ----
     for kind, label in ((0, "int64"), (1, "float64")) if "groupby" in legs else ():
@@ -174,6 +175,55 @@ def main():
                                     "roofline": {"bound": "hbm", "achieved": alg / (k / 1e3) / 1e9 if k else None, "peak": peak,
                                                  "frac": (alg / (k / 1e3) / 1e9 / peak) if k else None, "algorithmic_bytes_per_launch": alg},
                                     "kernels": kern}
+    if "protobuf" in legs:
+        # ---- protobuf_to_arrow / arrow_to_protobuf of schema S, and the JSON codec pair on the same records ----
+        import shutil
+        import tempfile
+
+        from arkflow_b200.processor import ArrowToJsonProcessor, ArrowToProtobufProcessor, ProtobufToArrowProcessor
+        from oracle.synth import synth_batch
+
+        m = min(n, 1 << 22)
+        pdir = tempfile.mkdtemp(prefix="ark_bench_proto_")  # nothing is written into the tree
+        with open(os.path.join(pdir, "s.proto"), "w") as f:
+            f.write('syntax = "proto3";\npackage bench;\nmessage S { int64 timestamp = 1; double value = 2; string sensor = 3; }\n')
+        cfg = {"proto_inputs": [pdir], "message_type": "bench.S"}
+        rows = F.DeviceBatch.from_arrow(synth_batch(m, value_kind=1, key_space=args.keys))
+        codecs = {"protobuf": (ArrowToProtobufProcessor(cfg), ProtobufToArrowProcessor(cfg),
+                               ["protobuf_encode_measure_kernel", "protobuf_encode_write_kernel"], ["protobuf_decode_kernel", "protobuf_strings_kernel"]),
+                  "json": (ArrowToJsonProcessor({}), JsonToArrowProcessor({}),
+                           ["arrow_to_json_measure_kernel", "arrow_to_json_write_kernel"], ["json_parse_kernel", "json_strings_kernel"])}
+        res = {"messages": m, "schema": "timestamp Int64, value Float64, sensor Utf8 (12 B)"}
+        for name, (enc, dec, enc_k, dec_k) in codecs.items():
+            encoded = enc.process_device(rows)
+            value = [c for c in encoded.columns if c.name == "__value__"][0]
+            payload = F.DeviceBatch([value], m)
+            payload_bytes = int(value.offsets[-1].item())
+
+            def estep():
+                enc.process_device(rows).close()
+
+            def dstep():
+                dec.process_device(payload).close()
+
+            wall_e, kern_e = timed(estep, enc_k)
+            wall_d, kern_d = timed(dstep, dec_k)
+            k_e = sum(kern_e[k]["avg_ms"] for k in enc_k)
+            k_d = kern_d[dec_k[0]]["avg_ms"]
+            # encode: both passes read the 32 B/row of the columns (8 + 8 + 4 offset + 12 string bytes); the lengths (4 B/row)
+            # are written and read back; the messages are written once.  decode (parse kernel): offsets + payload bytes in,
+            # 8 + 8 B of values + the sensor span (8 B source, 4 B length) out per message.
+            alg_e = 2 * m * 32 + 2 * m * 4 + payload_bytes
+            alg_d = m * 4 + payload_bytes + m * (8 + 8 + 12)
+            roof = lambda alg, k: {"bound": "hbm", "achieved": alg / (k / 1e3) / 1e9 if k else None, "peak": peak,
+                                   "frac": (alg / (k / 1e3) / 1e9 / peak) if k else None, "algorithmic_bytes_per_launch": alg}
+            res[name] = {"payload_bytes_per_msg": payload_bytes / m,
+                         "encode": {"msgs_per_s_call": m / wall_e, "ms_per_call": wall_e * 1e3, "kernel_ms": k_e, "roofline": roof(alg_e, k_e), "kernels": kern_e},
+                         "decode": {"msgs_per_s_call": m / wall_d, "ms_per_call": wall_d * 1e3, "kernel_ms": k_d, "roofline": roof(alg_d, k_d), "kernels": kern_d}}
+            payload.close()
+            encoded.close()
+        results["protobuf_vs_json"] = res
+        shutil.rmtree(pdir, ignore_errors=True)
     print(json.dumps(results, indent=1))
     if args.out:
         with open(os.path.join(ROOT, args.out), "w") as f:
