@@ -56,14 +56,16 @@ _FIXED = {"int64": ("<i8", 8, "int64", pa.int64), "float64": ("<f8", 8, "float64
 
 
 class DeviceColumn:
-    """One column resident in HBM.  `data`/`offsets`/`validity` are torch CUDA tensors (or None)."""
+    """One column resident in HBM.  `data`/`offsets`/`validity` are torch CUDA tensors (or None).  `offset` is the
+    Arrow offset of a slice: the column's rows start at element / bit `offset` of those buffers."""
 
     def __init__(self, name: str, dtype: str, length: int, data, offsets=None, validity=None,
-                 null_count: int = 0, nullable: bool = True):
+                 null_count: int = 0, nullable: bool = True, offset: int = 0):
         assert dtype in _FMT, dtype
         self.name, self.dtype, self.length = name, dtype, int(length)
         self.data, self.offsets, self.validity = data, offsets, validity
         self.null_count, self.nullable = null_count, nullable
+        self.offset = int(offset)
 
 
 class _LazyBytes:
@@ -185,7 +187,7 @@ class DeviceBatch:
                         bufs.append((c.data.data_ptr() or None) if c.data is not None else None)
                 barr = (C.c_void_p * max(len(bufs), 1))(*bufs)
                 a = child_arrs[i]
-                a.length, a.null_count, a.offset = c.length, (c.null_count if c.validity is not None else 0), 0
+                a.length, a.null_count, a.offset = c.length, (c.null_count if c.validity is not None else 0), c.offset
                 a.n_buffers, a.n_children = len(bufs), 0
                 a.buffers = C.cast(barr, C.POINTER(C.c_void_p))
                 child_ptrs[i] = C.pointer(a)
@@ -296,22 +298,28 @@ class DeviceBatch:
                 arrays.append(pa.nulls(n))
                 fields.append(pa.field(c.name, pa.null(), nullable=True))
                 continue
+            off = getattr(c, "offset", 0)
             if c.dtype in _FIXED:
                 t = _FIXED[c.dtype][3]()
-                arr = pa.Array.from_buffers(t, n, [vbuf, pa.py_buffer(c.data.cpu().numpy().tobytes())], null_count=nulls)
+                arr = pa.Array.from_buffers(t, n, [vbuf, pa.py_buffer(c.data.cpu().numpy().tobytes())], null_count=nulls, offset=off)
             elif c.dtype == "bool":
-                arr = pa.Array.from_buffers(pa.bool_(), n, [vbuf, pa.py_buffer(c.data.cpu().numpy().tobytes())], null_count=nulls)
+                arr = pa.Array.from_buffers(pa.bool_(), n, [vbuf, pa.py_buffer(c.data.cpu().numpy().tobytes())], null_count=nulls, offset=off)
             else:
                 t = pa.utf8() if c.dtype == "utf8" else pa.binary()
                 arr = pa.Array.from_buffers(t, n, [vbuf, pa.py_buffer(c.offsets.cpu().numpy().tobytes()),
-                                                   pa.py_buffer(c.data.cpu().numpy().tobytes())], null_count=nulls)
+                                                   pa.py_buffer(c.data.cpu().numpy().tobytes())], null_count=nulls, offset=off)
             arrays.append(arr)
             fields.append(pa.field(c.name, arr.type, nullable=c.nullable))
         return pa.RecordBatch.from_arrays(arrays, schema=pa.schema(fields))
 
     @staticmethod
-    def from_arrow(rb: pa.RecordBatch, device="cuda") -> "DeviceBatch":
-        """Upload a pyarrow RecordBatch with torch (test helper; the product H2D path is the C ABI)."""
+    def from_arrow(rb: pa.RecordBatch, device="cuda", keep_offsets: bool = False) -> "DeviceBatch":
+        """Upload a pyarrow RecordBatch with torch (test helper; the product H2D path is the C ABI).
+
+        Sliced columns are normalised to offset 0, unless keep_offsets: then each sliced column's parent buffers are
+        uploaded whole and exported with the slice's Arrow offset, as a producer that slices device batches (arrow-rs
+        RecordBatch::slice) hands them over: data pointers not 16-byte aligned, offsets[0] != 0, validity and Boolean
+        bits that start inside a byte."""
         import numpy as np
         import torch
 
@@ -327,23 +335,24 @@ class DeviceBatch:
         cols = []
         for name, arr in zip(rb.schema.names, rb.columns):
             f = rb.schema.field(name)
-            if arr.offset != 0:
+            if arr.offset != 0 and not keep_offsets:
                 arr = pa.concat_arrays([arr])  # normalise slices
+            off = arr.offset
             bufs = arr.buffers()
             n = len(arr)
             validity = up(bufs[0], np.uint8) if (bufs[0] is not None and arr.null_count) else None
             fixed = [k for k, v in _FIXED.items() if arr.type == v[3]()]
             if fixed:
                 dt = fixed[0]
-                data = up(bufs[1], np.dtype(_FIXED[dt][0]), n)
-                cols.append(DeviceColumn(name, dt, n, data, None, validity, arr.null_count, f.nullable))
+                data = up(bufs[1], np.dtype(_FIXED[dt][0]), off + n)
+                cols.append(DeviceColumn(name, dt, n, data, None, validity, arr.null_count, f.nullable, off))
             elif pa.types.is_boolean(arr.type):
-                cols.append(DeviceColumn(name, "bool", n, up(bufs[1], np.uint8), None, validity, arr.null_count, f.nullable))
+                cols.append(DeviceColumn(name, "bool", n, up(bufs[1], np.uint8), None, validity, arr.null_count, f.nullable, off))
             elif pa.types.is_string(arr.type) or pa.types.is_binary(arr.type):
                 dt = "utf8" if pa.types.is_string(arr.type) else "binary"
-                offsets = up(bufs[1], np.int32, n + 1)
+                offsets = up(bufs[1], np.int32, off + n + 1)
                 data = up(bufs[2], np.uint8) if bufs[2] is not None else torch.empty(0, dtype=torch.uint8, device=device)
-                cols.append(DeviceColumn(name, dt, n, data, offsets, validity, arr.null_count, f.nullable))
+                cols.append(DeviceColumn(name, dt, n, data, offsets, validity, arr.null_count, f.nullable, off))
             else:
                 raise TypeError(f"unsupported Arrow type for device upload: {arr.type}")
         return DeviceBatch(cols, rb.num_rows)

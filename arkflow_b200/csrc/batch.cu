@@ -38,7 +38,7 @@ bool timing_get(const char* name, double* ms, int64_t* n) {
 
 // Timed launches record an event pair and resolve it lazily (no synchronisation on the launch path):
 // ark_kernel_timing_get() is called after the caller has synchronised the device.
-struct PendingTiming { const char* name; cudaEvent_t e0, e1; };
+struct PendingTiming { const char* name; const char* also; cudaEvent_t e0, e1; };
 static std::vector<PendingTiming> g_pending;
 static std::vector<cudaEvent_t> g_event_pool;
 
@@ -57,13 +57,14 @@ static void resolve_pending_locked() {
     float ms = 0;
     if (cudaEventSynchronize(p.e1) == cudaSuccess && cudaEventElapsedTime(&ms, p.e0, p.e1) == cudaSuccess) {
       auto& e = g_timing_map[p.name]; e.ms += ms; e.n += 1;
+      if (p.also) { auto& a = g_timing_map[p.also]; a.ms += ms; a.n += 1; }
     } else cudaGetLastError();
     g_event_pool.push_back(p.e0); g_event_pool.push_back(p.e1);
   }
   g_pending.clear();
 }
 
-KernelTimer::KernelTimer(const char* n, cudaStream_t s) : name(n), stream(s) {
+KernelTimer::KernelTimer(const char* n, cudaStream_t s, const char* a) : name(n), also(a), stream(s) {
   note_launch(n);
   if (g_timing.load(std::memory_order_relaxed)) {
     e0 = take_event(); e1 = take_event();
@@ -74,7 +75,7 @@ KernelTimer::~KernelTimer() {
   if (e0) {
     cudaEventRecord(e1, stream);
     std::lock_guard<std::mutex> l(g_timing_mu);
-    g_pending.push_back({name, e0, e1});
+    g_pending.push_back({name, also, e0, e1});
   }
 }
 

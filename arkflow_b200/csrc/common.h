@@ -35,9 +35,11 @@ void set_last_error(const std::string& msg);
 // ---- kernel launch accounting (ark_kernel_launch_count / ark_kernel_timing_*) ----
 void note_launch(const char* name);
 struct KernelTimer {  // RAII: records CUDA events around one launch when timing is enabled
-  KernelTimer(const char* name, cudaStream_t s);
+  // `also`: a second name the same launch is recorded under (a group of kernels timed together, e.g. hash_agg_kernel)
+  KernelTimer(const char* name, cudaStream_t s, const char* also = nullptr);
   ~KernelTimer();
   const char* name;
+  const char* also;
   cudaStream_t stream;
   cudaEvent_t e0 = nullptr, e1 = nullptr;
 };

@@ -135,7 +135,13 @@ __global__ void __launch_bounds__(AGG_THREADS) hash_agg_kernel(const __grid_cons
       bool valid = ok;
       if (ok && A.kind != ACC_COUNT_STAR) {
         if (A.arg_prog >= 0) { VmVal v = vm_eval(P.progs[A.arg_prog], P.cols, row, &err); bits = v.bits; valid = v.valid; }
-        else { const ColView& c = P.cols[A.arg_slot]; valid = col_valid(c, row); bits = valid ? __ldcs((const unsigned long long*)c.data + row) : 0; }
+        else {
+          // COUNT(x) needs x's validity only: x may be a Utf8 / Binary / Boolean column, whose data buffer does not hold
+          // 8-byte values
+          const ColView& c = P.cols[A.arg_slot];
+          valid = col_valid(c, row);
+          bits = valid && A.kind != ACC_COUNT ? __ldcs((const unsigned long long*)c.data + row) : 0;
+        }
       }
       unsigned long long* dst = tbl_acc(P.table, uniform ? slot0 : slot, a, bstride);
       switch (A.kind) {
@@ -263,6 +269,8 @@ __global__ void agg_finalize_kernel(int op, const unsigned long long* a, const u
 
 template <int PRED>
 void launch_agg(const AggParams& P, int64_t n, cudaStream_t stream) {
+  // hash_agg_kernel also counts the staged and register-prefetch launches (hash_agg_stream.cu), which carry their own
+  // names too: this kernel's launches are hash_agg_kernel minus those two
   KernelTimer t("hash_agg_kernel", stream);
   const int grid = (int)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, (int64_t)AGG_THREADS), sm_count() * 8));
   hash_agg_kernel<PRED><<<grid, AGG_THREADS, 0, stream>>>(P);

@@ -53,6 +53,9 @@ enum AccKind : int32_t {
   ACC_MIN_F64, ACC_MAX_F64,  // on the totalOrder key
 };
 
+// COUNT(*) has no argument and COUNT(x) needs only x's validity; every other accumulator reads x's 8-byte values
+__host__ __device__ inline bool acc_reads_values(int kind) { return kind != ACC_COUNT_STAR && kind != ACC_COUNT; }
+
 enum KeyKind : int32_t { KEY_NONE = 0, KEY_INT64 = 1, KEY_BYTES = 2, KEY_BOOL = 3, KEY_PAIR = 4 /* two key columns */ };
 
 constexpr int AGG_MAX_ACC = 8;

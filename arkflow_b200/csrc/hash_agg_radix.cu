@@ -265,7 +265,11 @@ bool launch_hash_agg_radix(const AggParams& P, unsigned long long capacity, int3
     R.acc_v[a] = -1;
     if (A.arg_prog >= 0) return false;
     if (A.kind == ACC_COUNT_STAR) continue;
+    // an argument with a validity buffer declines the path: the records carry no validity.  COUNT(x) of an argument
+    // without one (nullable by schema only) counts every row and records no values: x may be a Utf8 / Binary / Boolean
+    // column, which holds no 8-byte values
     if (P.cols[A.arg_slot].validity) return false;
+    if (!acc_reads_values(A.kind)) continue;
     int vi = -1;
     for (int v = 0; v < R.nv; ++v) if (R.v_slot[v] == A.arg_slot) vi = v;
     if (vi < 0) { if (R.nv == 2) return false; vi = R.nv; R.v_slot[R.nv++] = A.arg_slot; }

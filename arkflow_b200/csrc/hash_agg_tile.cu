@@ -202,13 +202,16 @@ __global__ void __launch_bounds__(HT_THREADS, 3) hash_agg_tile_kernel(const __gr
       unsigned valid = ok;
       if (A.kind != ACC_COUNT_STAR) {
         const ColView& c = P.cols[A.arg_slot];
-        const unsigned long long* src = (const unsigned long long*)c.data + row0 + lr0;
-        if (full_rows && (reinterpret_cast<uintptr_t>(src) & 15) == 0) {
-          asm volatile("ld.global.cs.v2.u64 {%0, %1}, [%2];" : "=l"(av[0]), "=l"(av[1]) : "l"(src));
-          asm volatile("ld.global.cs.v2.u64 {%0, %1}, [%2];" : "=l"(av[2]), "=l"(av[3]) : "l"(src + 2));
-        } else {
+        // COUNT(x) reads x's validity only (x may be Utf8 / Binary / Boolean: no 8-byte values to load)
+        if (A.kind != ACC_COUNT) {
+          const unsigned long long* src = (const unsigned long long*)c.data + row0 + lr0;
+          if (full_rows && (reinterpret_cast<uintptr_t>(src) & 15) == 0) {
+            asm volatile("ld.global.cs.v2.u64 {%0, %1}, [%2];" : "=l"(av[0]), "=l"(av[1]) : "l"(src));
+            asm volatile("ld.global.cs.v2.u64 {%0, %1}, [%2];" : "=l"(av[2]), "=l"(av[3]) : "l"(src + 2));
+          } else {
 #pragma unroll
-          for (int j = 0; j < 4; ++j) av[j] = (lr0 + j < rows) ? src[j] : 0;
+            for (int j = 0; j < 4; ++j) av[j] = (lr0 + j < rows) ? src[j] : 0;
+          }
         }
         if (c.validity) {
 #pragma unroll

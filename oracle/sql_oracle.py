@@ -784,12 +784,33 @@ def _empty_schema_batch() -> pa.RecordBatch:
     return pa.RecordBatch.from_arrays([], schema=pa.schema([]))
 
 
+def sum_exact(xs: list[float]) -> float:
+    """The IEEE-754 sum of `xs` without intermediate rounding, total over non-finite inputs: NaN when a NaN or both
+    infinities occur, ±inf when infinities of one sign occur, else the correctly rounded exact sum — ±inf when that
+    leaves the double range.  (Any summation order yields the same NaN / ±inf in the non-finite cases.)"""
+    if any(math.isnan(x) for x in xs):
+        return math.nan
+    pinf, ninf = math.inf in xs, -math.inf in xs
+    if pinf or ninf:
+        return math.nan if pinf and ninf else (math.inf if pinf else -math.inf)
+    try:
+        return math.fsum(xs)
+    except OverflowError:  # fsum gives up once a partial sum leaves the double range: sum exactly, round once
+        from fractions import Fraction
+
+        s = sum(Fraction(x) for x in xs)
+        try:
+            return float(s)  # int / int true division: correctly rounded
+        except OverflowError:
+            return math.inf if s > 0 else -math.inf
+
+
 def group_sum_exact(values: np.ndarray, codes: np.ndarray, k: int) -> list[float]:
-    """Correctly-rounded per-group Float64 sums (math.fsum) — the reference point of the tolerance."""
+    """Correctly-rounded per-group Float64 sums (sum_exact) — the reference point of the tolerance."""
     order = np.argsort(codes, kind="stable")
     sv, sc = values[order], codes[order]
     bounds = np.searchsorted(sc, np.arange(k + 1))
-    return [math.fsum(sv[bounds[i]:bounds[i + 1]].tolist()) for i in range(k)]
+    return [sum_exact(sv[bounds[i]:bounds[i + 1]].tolist()) for i in range(k)]
 
 
 def sql_process(rb: pa.RecordBatch, query: str, table_name: str = "flow") -> Optional[pa.RecordBatch]:

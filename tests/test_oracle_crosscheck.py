@@ -2,6 +2,8 @@
 the SQL subset where DataFusion's and Arrow C++'s semantics coincide (Int64 arithmetic without overflow, Int64 /
 Utf8 comparisons, inner equi-join, SUM / COUNT / MIN / MAX / AVG over Int64).  This does not pin the oracle to the
 reference (only the reference's own assertions do, tests/golden/), but it catches slips in the restatement."""
+import math
+
 import numpy as np
 import pyarrow as pa
 import pyarrow.compute as pc
@@ -136,3 +138,51 @@ def test_json_decode_matches_arrow_json_reader():
     assert got.schema.names == want.schema.names
     for name in want.schema.names:
         assert got.column(name).to_pylist() == want[name].to_pylist(), name
+
+
+# ---- non-finite float sums: group_sum_exact is total (NaN / ±inf where math.fsum raises) -----------------------------
+INF, NAN = float("inf"), float("nan")
+
+
+@pytest.mark.parametrize("xs, want", [
+    ([INF, -INF], NAN),                   # fsum: ValueError (-inf + inf)
+    ([1.0, INF, 2.0, -INF], NAN),
+    ([NAN, 1.0], NAN),
+    ([-NAN, INF], NAN),
+    ([INF, 1e300, INF], INF),
+    ([-INF, -5e-324, 3.0], -INF),
+    ([1.7e308, 1.7e308], INF),            # fsum: OverflowError (the exact sum is out of range)
+    ([-1.7e308, -1.7e308, 1.0], -INF),
+    ([1.7e308, 1.7e308, -1.7e308], 1.7e308),   # a partial sum leaves the range, the exact sum does not
+    ([1e300, 5e-324, -1e300], 5e-324),
+    ([-0.0], -0.0),
+    ([], 0.0),
+])
+def test_group_sum_exact_non_finite(xs, want):
+    from fractions import Fraction
+
+    from oracle.sql_oracle import group_sum_exact
+
+    got = group_sum_exact(np.array(xs, np.float64), np.zeros(len(xs), np.int64), 1)[0]
+    if math.isnan(want):
+        assert math.isnan(got)
+    else:
+        assert got == want, (xs, got)
+        if math.isfinite(want) and xs:
+            assert Fraction(got) == Fraction(want)
+
+
+def test_sql_sum_avg_over_non_finite_groups():
+    """SUM / AVG over groups holding both infinities, NaN or an out-of-range exact sum: the oracle answers where it used to
+    raise, and groups of finite values keep the correctly rounded sum."""
+    k = ["both", "both", "nan", "nan", "pinf", "pinf", "big", "big", "fin", "fin", "null"]
+    v = [INF, -INF, NAN, 2.0, INF, 1e300, 1.7e308, 1.7e308, 0.1, 0.2, None]
+    rb = pa.record_batch({"k": pa.array(k), "v": pa.array(v, pa.float64())})
+    got = sql_process(rb, "SELECT k, SUM(v), AVG(v), COUNT(v) FROM flow GROUP BY k")
+    d = {r["k"]: (r["sum(flow.v)"], r["avg(flow.v)"], r["count(flow.v)"]) for r in got.to_pylist()}
+    assert math.isnan(d["both"][0]) and math.isnan(d["both"][1])
+    assert math.isnan(d["nan"][0]) and math.isnan(d["nan"][1])
+    assert d["pinf"][:2] == (INF, INF)
+    assert d["big"][:2] == (INF, INF)
+    assert d["fin"] == (0.30000000000000004, 0.15000000000000002, 2)
+    assert d["null"] == (None, None, 0)

@@ -12,6 +12,7 @@ import pyarrow as pa
 import pyarrow.compute  # noqa: F401
 import pytest
 
+from agg_util import float_sum_bound, float_sum_mismatches
 from arkflow_b200.arrow_ffi import DeviceBatch
 from arkflow_b200.processor import ArkError, MessageBatch, SqlProcessor
 from oracle.sql_oracle import sql_process
@@ -67,9 +68,9 @@ def check_agg(rb, query, key_cols, float_cols=(), abs_sums=None, counts=None):
                         assert (gv is None) == (wv is None)
                         if wv is None:
                             continue
-                        bound = 2 * max(n_rows - 1, 1) * 2.0 ** -53 * (s_abs if s_abs is not None else abs(wv) * n_rows) + 1e-300
-                        if want.schema.names[i].startswith("avg"):
-                            bound = bound + abs(wv) * 2.0 ** -52
+                        # the bound over the whole batch, not divided by the row count for AVG
+                        bound = float_sum_bound(n_rows, s_abs if s_abs is not None else abs(wv) * n_rows, wv) + \
+                            (abs(wv) * 2.0 ** -52 if want.schema.names[i].startswith("avg") else 0.0)
                         assert abs(gv - wv) <= bound, (want.schema.names[i], gv, wv, bound)
             continue
         gd, wd = rows_as_dict(got, key_cols), rows_as_dict(want, key_cols)
@@ -79,10 +80,8 @@ def check_agg(rb, query, key_cols, float_cols=(), abs_sums=None, counts=None):
                 gv, wv = gd[k][n], wd[k][n]
                 if n in float_cols and wv is not None and gv is not None:
                     ng = counts[k] if counts else 1
-                    bound = 2 * max(ng - 1, 1) * 2.0 ** -53 * (abs_sums[k] if abs_sums else abs(wv)) + 1e-300
-                    if n.startswith("avg"):
-                        bound = bound / max(ng, 1) + abs(wv) * 2.0 ** -52
-                    assert abs(gv - wv) <= bound, (k, n, gv, wv, bound)
+                    bad = float_sum_mismatches([gv], [wv], ng, abs_sums[k] if abs_sums else abs(wv), avg=n.startswith("avg"))
+                    assert len(bad) == 0, (k, n, gv, wv)
                 else:
                     assert gv == wv, (k, n, gv, wv)
     return want

@@ -4,6 +4,8 @@ Mirrors the reference's in-file tests of the sql processor
 (crates/arkflow-plugin/src/processor/sql.rs:257-425) and widens them with value checks:
 integer / byte / index work must be bit-exact.
 """
+import os
+
 import numpy as np
 import pyarrow as pa
 import pytest
@@ -264,6 +266,54 @@ def test_sliced_input_arrays(gpu):
     rb = synth_batch(10_000, key_space=33).slice(1237, 5001)
     check(rb, "SELECT sensor, value FROM flow WHERE value >= 10")
     check(rb, "SELECT * FROM flow")
+
+
+_DEVICE_SLICES = '''
+import sys
+sys.path.insert(0, %r)
+import os
+
+import numpy as np
+import pyarrow as pa
+from arkflow_b200 import _lib as L
+from arkflow_b200.arrow_ffi import DeviceBatch
+from arkflow_b200.processor import SqlProcessor, _check
+from oracle.sql_oracle import sql_process
+_check(L.lib().ark_b200_init(0))
+rng = np.random.default_rng(17)
+n = 70_000
+v = rng.integers(0, 20, n + 1237)
+rb = pa.record_batch({
+    "value": pa.array(v, pa.int64(), mask=rng.random(n + 1237) < 0.1),
+    "sensor": pa.array(["s%%d" %% x * int(x %% 4) for x in v], pa.utf8(), mask=rng.random(n + 1237) < 0.2),
+    "blob": pa.array([b"\\x00b%%d" %% x for x in v], pa.binary()),
+    "flag": pa.array(v %% 3 == 0, pa.bool_(), mask=rng.random(n + 1237) < 0.15),
+    "f": pa.array(rng.uniform(-1, 1, n + 1237), pa.float64()),
+})
+queries = ["SELECT sensor, value FROM flow WHERE value >= 10", "SELECT * FROM flow WHERE f < 0.25", "SELECT * FROM flow",
+           "SELECT value + 1, blob, flag FROM flow WHERE flag", "SELECT sensor, f FROM flow WHERE value IS NULL OR f > 0.5"]
+for off in (1, 3, 7, 1237):
+    for m in (1, 1000, n):
+        sl = rb.slice(off, m)
+        want_rb = pa.RecordBatch.from_arrays([pa.concat_arrays([c]) for c in sl.columns], schema=sl.schema)
+        for q in queries:
+            got = SqlProcessor({"query": q}).process_device(DeviceBatch.from_arrow(sl, keep_offsets=True)).to_arrow()
+            assert got.equals(sql_process(want_rb, q)), (off, m, q)
+print("SLICES_OK")
+''' % os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+@pytest.mark.parametrize("env", [{}, {"ARK_FP_IMPL": "3"}])
+def test_device_sliced_inputs(gpu, env):
+    """Device batches whose columns are Arrow slices, as a producer that slices device batches hands them over: Int64 data
+    8 bytes past a 16-byte boundary, offsets 4-aligned with offsets[0] != 0, validity and Boolean bits that start inside a
+    byte.  The default tile kernel and the ring kernel (ARK_FP_IMPL=3, every input staged by TMA).  Subprocess: the knob is
+    read once per process."""
+    import subprocess
+    import sys
+
+    r = subprocess.run([sys.executable, "-c", _DEVICE_SLICES], capture_output=True, text=True, timeout=300, env=dict(os.environ, **env))
+    assert r.returncode == 0 and "SLICES_OK" in r.stdout, r.stdout[-1500:] + r.stderr[-1500:]
 
 
 def test_ragged_and_long_strings(gpu):
