@@ -15,19 +15,21 @@
 //               Deviations from DataFusion's readers: the JSON schema is inferred from the first record (as the
 //               json_to_arrow processor does; DataFusion samples 1000), CSV types from the first 1000 rows with the
 //               types Int64 / Float64 / Boolean / Utf8 (dates stay strings), quoted CSV fields may not contain line
-//               breaks.
+//               breaks.  A CSV column is Int64 when its sample values are decimal integers within the i64 range, and
+//               Float64 when they are decimals or nan / inf / infinity (any case, optional sign; Arrow's reader
+//               accepts these spellings too); Float64 values are correctly rounded.
 #include <sys/stat.h>
 
 #include <chrono>
 #include <cstdio>
 #include <thread>
 
-#include <math_constants.h>
 #include <thrust/iterator/counting_iterator.h>
 
 #include <cub/device/device_scan.cuh>
 #include <cub/device/device_select.cuh>
 
+#include "decimal.cuh"
 #include "engine.h"
 #include "json_mini.h"
 
@@ -120,7 +122,9 @@ struct CsvParams {
   int32_t* error;                    // [0] = 1 bad number / 2 wrong field count, [1] = row
 };
 
-__device__ inline bool csv_parse_i64(const uint8_t* p, int len, long long* out) {
+// The host's type inference (csv_infer_type) calls the same two grammar tests as the kernel, so a column inferred
+// Int64 / Float64 from its sample rows parses on the device.
+__host__ __device__ inline bool csv_parse_i64(const uint8_t* p, int len, long long* out) {
   if (len <= 0) return false;
   int i = 0;
   bool neg = false;
@@ -138,46 +142,25 @@ __device__ inline bool csv_parse_i64(const uint8_t* p, int len, long long* out) 
   return true;
 }
 
-// decimal → double: exact for ≤ 15 significant digits and |exp10| ≤ 22 (two correctly rounded operations), otherwise
-// within 1 ulp (same contract as the JSON number path, DESIGN.md §4.5)
+// [+-]? then nan / inf / infinity in any case, as Arrow's CSV reader spells them → the f64 bits.  NaN keeps no sign.
+__host__ __device__ inline bool csv_special_f64(const uint8_t* p, int len, unsigned long long* bits) {
+  int i = (len > 0 && (p[0] == '-' || p[0] == '+')) ? 1 : 0;
+  const bool neg = i == 1 && p[0] == '-';
+  auto word = [&](const char* w, int n) {
+    if (len - i != n) return false;
+    for (int k = 0; k < n; ++k) if ((p[i + k] | 32) != w[k]) return false;
+    return true;
+  };
+  if (word("nan", 3)) { *bits = 0x7FF8000000000000ull; return true; }
+  if (word("inf", 3) || word("infinity", 8)) { *bits = neg ? 0xFFF0000000000000ull : 0x7FF0000000000000ull; return true; }
+  return false;
+}
+
+// decimal → double, correctly rounded (decimal.cuh, the routine the JSON decoder uses), or one of the special spellings
 __device__ inline bool csv_parse_f64(const uint8_t* p, int len, double* out) {
-  if (len <= 0) return false;
-  int i = 0;
-  bool neg = false;
-  if (p[0] == '-' || p[0] == '+') { neg = p[0] == '-'; i = 1; }
-  if (len - i == 3 && (p[i] | 32) == 'n' && (p[i + 1] | 32) == 'a' && (p[i + 2] | 32) == 'n') { *out = __longlong_as_double(0x7FF8000000000000ll); return true; }
-  if (len - i == 3 && (p[i] | 32) == 'i' && (p[i + 1] | 32) == 'n' && (p[i + 2] | 32) == 'f') { *out = neg ? -CUDART_INF : CUDART_INF; return true; }
-  unsigned long long mant = 0;
-  int digits = 0, exp10 = 0;
-  bool any = false;
-  for (; i < len && (unsigned)(p[i] - '0') <= 9; ++i) { any = true; if (digits < 19) { mant = mant * 10 + (p[i] - '0'); if (mant) ++digits; } else ++exp10; }
-  if (i < len && p[i] == '.') {
-    ++i;
-    for (; i < len && (unsigned)(p[i] - '0') <= 9; ++i) { any = true; if (digits < 19) { mant = mant * 10 + (p[i] - '0'); if (mant) ++digits; --exp10; } }
-  }
-  if (!any) return false;
-  if (i < len && (p[i] | 32) == 'e') {
-    ++i;
-    bool eneg = false;
-    if (i < len && (p[i] == '-' || p[i] == '+')) { eneg = p[i] == '-'; ++i; }
-    if (i >= len) return false;
-    int e = 0;
-    for (; i < len; ++i) { const unsigned d = (unsigned)p[i] - '0'; if (d > 9) return false; if (e < 10000) e = e * 10 + (int)d; }
-    exp10 += eneg ? -e : e;
-  }
-  if (i != len) return false;
-  double v = (double)mant;
-  if (mant != 0) {
-    if (exp10 > 330) v = CUDART_INF;
-    else if (exp10 < -360) v = 0.0;
-    else {
-      int e = exp10;
-      while (e > 0) { const int s = e > 22 ? 22 : e; v *= pow(10.0, (double)s); e -= s; }
-      while (e < 0) { const int s = -e > 22 ? 22 : -e; v /= pow(10.0, (double)s); e += s; }
-    }
-  }
-  *out = neg ? -v : v;
-  return true;
+  unsigned long long bits;
+  if (csv_special_f64(p, len, &bits)) { *out = __longlong_as_double((long long)bits); return true; }
+  return decimal_to_f64(p, len, out);
 }
 
 // One thread per row: split at the delimiter (quoted fields may hold delimiters and "" escapes), convert per type.
@@ -415,8 +398,10 @@ std::vector<std::string> split_csv_line(const std::string& line, char delim) {
 
 int csv_infer_type(const std::string& f, int cur) {  // -1 = no evidence yet (only empty fields)
   if (f.empty()) return cur;
-  auto is_int = [&] { size_t i = (f[0] == '-' || f[0] == '+') ? 1 : 0; if (i >= f.size()) return false; for (; i < f.size(); ++i) if (!isdigit((unsigned char)f[i])) return false; return f.size() <= 19; };
-  auto is_float = [&] { char* e = nullptr; errno = 0; strtod(f.c_str(), &e); return e && *e == 0 && !isspace((unsigned char)f[0]); };
+  const uint8_t* p = (const uint8_t*)f.data();
+  const int n = (int)f.size();
+  auto is_int = [&] { long long v; return csv_parse_i64(p, n, &v); };  // digits, and a value that fits i64
+  auto is_float = [&] { unsigned long long b; DecimalScan d; return csv_special_f64(p, n, &b) || decimal_scan(p, n, &d); };
   auto is_bool = [&] { std::string l; for (char c : f) l += (char)tolower((unsigned char)c); return l == "true" || l == "false"; };
   int t = is_int() ? CSV_I64 : (is_float() ? CSV_F64 : (is_bool() ? CSV_BOOL : CSV_STR));
   if (cur < 0) return t;

@@ -21,7 +21,7 @@
 #include "engine.h"
 #include "tma.cuh"
 #include "json_mini.h"
-#include "pow10_table.h"
+#include "decimal.cuh"
 
 namespace ark {
 
@@ -160,65 +160,8 @@ __device__ bool skip_value(Cursor& c, int) {
   return depth == 0;
 }
 
-__constant__ double kPow10[23] = {1e0, 1e1, 1e2, 1e3, 1e4, 1e5, 1e6, 1e7, 1e8, 1e9, 1e10, 1e11, 1e12, 1e13, 1e14, 1e15,
-                                  1e16, 1e17, 1e18, 1e19, 1e20, 1e21, 1e22};
-
-// decimal text → f64.  Exact (correctly rounded) on Clinger's fast path: ≤ 19 significant digits
-// with mantissa < 2^53 and |exp10| ≤ 22; otherwise scaled in double (≤ 1 ulp off; see DESIGN.md).
-__device__ bool parse_f64(const uint8_t* s, int len, double* out) {
-  int i = 0;
-  bool neg = false;
-  if (i < len && s[i] == '-') { neg = true; ++i; }
-  else if (i < len && s[i] == '+') ++i;
-  unsigned long long mant = 0;
-  int digits = 0, exp10 = 0;
-  bool any = false;
-  for (; i < len && s[i] >= '0' && s[i] <= '9'; ++i) {
-    any = true;
-    if (digits < 19) { mant = mant * 10 + (s[i] - '0'); if (mant) ++digits; }
-    else ++exp10;
-  }
-  if (i < len && s[i] == '.') {
-    ++i;
-    for (; i < len && s[i] >= '0' && s[i] <= '9'; ++i) {
-      any = true;
-      if (digits < 19) { mant = mant * 10 + (s[i] - '0'); if (mant) ++digits; --exp10; }
-    }
-  }
-  if (!any) return false;
-  if (i < len && (s[i] == 'e' || s[i] == 'E')) {
-    ++i;
-    bool eneg = false;
-    if (i < len && (s[i] == '+' || s[i] == '-')) { eneg = s[i] == '-'; ++i; }
-    int e = 0; bool eany = false;
-    for (; i < len && s[i] >= '0' && s[i] <= '9'; ++i) { eany = true; if (e < 100000) e = e * 10 + (s[i] - '0'); }
-    if (!eany) return false;
-    exp10 += eneg ? -e : e;
-  }
-  if (i != len) return false;
-  double v;
-  if (mant == 0) v = 0.0;
-  else if (mant < (1ull << 53) && exp10 >= -22 && exp10 <= 22) {
-    v = (double)mant;
-    v = exp10 < 0 ? v / kPow10[-exp10] : v * kPow10[exp10];
-  } else if (exp10 > ARK_POW10_MAX) v = __longlong_as_double(0x7FF0000000000000ll);  // overflow → inf
-  else if (exp10 < ARK_POW10_MIN) v = 0.0;
-  else {
-    // 64-bit mantissa × 64-bit truncated power of ten → 128-bit product, top 64 bits + sticky → f64
-    // (round-to-nearest-even by the integer→double conversion).  Within 1 ulp; exact unless the
-    // product lies within 2^-63 of a rounding boundary.
-    const int lz = __clzll((long long)mant);
-    const unsigned long long w = mant << lz;
-    const unsigned long long pm = kPow10Mant[exp10 - ARK_POW10_MIN];
-    unsigned long long hi = __umul64hi(w, pm), lo = w * pm;
-    int e2 = (int)kPow10Exp2[exp10 - ARK_POW10_MIN] - lz + 64;
-    if (!(hi >> 63)) { hi = (hi << 1) | (lo >> 63); lo <<= 1; e2 -= 1; }
-    if (lo) hi |= 1;
-    v = ldexp((double)hi, e2);
-  }
-  *out = neg ? -v : v;
-  return true;
-}
+// JSON number text (or the body of a quoted number) → f64, correctly rounded (decimal.cuh)
+__device__ bool parse_f64(const uint8_t* s, int len, double* out) { return decimal_to_f64(s, len, out); }
 
 // JSON number text → i64 as arrow-json's ParseJsonNumber does: integer parse, else f64 then NumCast.
 __device__ bool parse_i64(const uint8_t* s, int len, long long* out) {

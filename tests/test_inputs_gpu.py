@@ -184,9 +184,9 @@ def test_file_csv_scan_matches_arrow_csv(gpu, tmp_path):
     assert [str(t) for t in table.schema.types] == ["int64", "int64", "double", "bool", "string"]
     for name in ("id", "value", "flag", "name"):
         assert table.column(name).to_pylist() == want.column(name).to_pylist(), name
-    g, w = table.column("score").to_pylist(), want.column("score").to_pylist()
-    assert [x is None for x in g] == [x is None for x in w]
-    assert all(a == b or abs(a - b) <= abs(b) * 2.3e-16 for a, b in zip(g, w) if a is not None)  # ≤ 1 ulp (DESIGN.md)
+    g, w = table.column("score"), want.column("score")
+    assert [x is None for x in g.to_pylist()] == [x is None for x in w.to_pylist()]
+    assert g.fill_null(0.0).to_numpy().view(np.uint64).tolist() == w.fill_null(0.0).to_numpy().view(np.uint64).tolist()  # correctly rounded
 
 
 def test_file_errors(gpu, tmp_path):

@@ -21,7 +21,7 @@ def run(mb, cfg=None, device=False):
     return p.process(mb).batches[0].record_batch
 
 
-def check(payloads, cfg=None, approx=()):
+def check(payloads, cfg=None):
     mb = MessageBatch.new_binary(payloads)
     inc = set(cfg["fields_to_include"]) if cfg and "fields_to_include" in cfg else None
     want = json_to_arrow(mb.record_batch, (cfg or {}).get("value_field", "__value__"), inc)
@@ -32,11 +32,9 @@ def check(payloads, cfg=None, approx=()):
         for name in want.schema.names:
             g, w = got.column(name), want.column(name)
             assert g.type == w.type, (name, g.type, w.type)
-            if name in approx:
-                for a, b in zip(g.to_pylist(), w.to_pylist()):
-                    assert (a is None) == (b is None) and (a is None or abs(a - b) <= abs(b) * 2.3e-16)
-            else:
-                assert g.to_pylist() == w.to_pylist(), name
+            assert g.to_pylist() == w.to_pylist(), name
+            if g.type == pa.float64():  # and the bits: -0.0 == 0.0 in Python
+                assert g.fill_null(0.0).to_numpy().view(np.uint64).tolist() == w.fill_null(0.0).to_numpy().view(np.uint64).tolist(), name
     return want
 
 
@@ -50,7 +48,7 @@ def test_generate_example_payloads(gpu):
 def test_basic_types_scalar_fields(gpu):
     # json.rs:170-207, scalar fields (the full record: test_reference_basic_types_record_with_array_and_object)
     rec = {"null_field": None, "bool_field": True, "int_field": 42, "uint_field": 18446744073709551615, "float_field": 3.14, "string_field": "hello"}
-    out = check([json.dumps(rec).encode()], approx=("uint_field",))
+    out = check([json.dumps(rec).encode()])
     assert out.num_rows == 1 and out.num_columns == 6
     assert [str(t) for t in out.schema.types] == ["null", "bool", "int64", "double", "double", "string"]
 
@@ -211,9 +209,10 @@ def test_numbers(gpu):
     payloads = [json.dumps({"i": 1, "f": 1.5}).encode()]
     payloads += [b'{"i": %d, "f": %s}' % (i, f.encode()) for i, f in zip(ints + ints, floats + floats)]
     check(payloads)
-    # beyond the exact fast path: at most 1 ulp (documented in DESIGN.md)
-    hard = [b'{"f": 1.5}', b'{"f": 1.7976931348623157e308}', b'{"f": 123456789012345678901234567890}', b'{"f": 4.9e-324}', b'{"f": 0.30000000000000004}']
-    check(hard, approx=("f",))
+    # beyond Clinger's fast path: still correctly rounded (tests/test_number_parse_gpu.py covers the whole range)
+    hard = [b'{"f": 1.5}', b'{"f": 1.7976931348623157e308}', b'{"f": 123456789012345678901234567890}', b'{"f": 4.9e-324}', b'{"f": 0.30000000000000004}',
+            b'{"f": 3.246986519402559e+185}', b'{"f": 2.2250738585072011e-308}', b'{"f": -0.0}']
+    check(hard)
 
 
 def test_int_column_errors(gpu):
