@@ -1393,7 +1393,7 @@ bool launch_filter_project_tma(int64_t n_rows, const void* pred_in, int n_fixed_
         static const int cap_per_sm = [] { const char* e = getenv("ARK_FP_CTAS_PER_SM"); return e ? atoi(e) : 0; }();
         if (cap_per_sm > 0) occ = std::min(occ, cap_per_sm);
         const int grid = std::max(1, std::min(P.n_tiles, sms * occ));
-        KernelTimer t("filter_project_tma_kernel", stream);
+        KernelTimer t("filter_project_tma_kernel", stream, "filter_project_ring_kernel");
         void* args[] = {(void*)&P};
         ARK_CUDA(cudaLaunchKernel(fn, dim3(grid), dim3(dt + 32), args, smem, stream));
         return true;
@@ -1426,7 +1426,7 @@ bool launch_filter_project_tma(int64_t n_rows, const void* pred_in, int n_fixed_
     else return false;
 #undef ARK_TILE_FN
 #undef ARK_TILE_R
-    KernelTimer t("filter_project_tma_kernel", stream);
+    KernelTimer t("filter_project_tma_kernel", stream, "filter_project_tile_kernel");
     void* args[] = {(void*)&P};
     ARK_CUDA(cudaLaunchKernel(fn, dim3(P.n_tiles), dim3(dt + 32), args, smem, stream));
     return true;
@@ -1463,7 +1463,7 @@ bool launch_filter_project_tma(int64_t n_rows, const void* pred_in, int n_fixed_
     static const int cap_per_sm = [] { const char* e = getenv("ARK_FP_CTAS_PER_SM"); return e ? atoi(e) : 0; }();
     const int per_sm = cap_per_sm > 0 ? std::min(cap_per_sm, o) : o;
     const int grid = std::max(1, std::min(P.n_tiles, sms * per_sm));
-    KernelTimer t("filter_project_tma_kernel", stream);
+    KernelTimer t("filter_project_tma_kernel", stream, "filter_project_pipe_kernel");
     void* args[] = {(void*)&P};
     ARK_CUDA(cudaLaunchKernel(fn, dim3(grid), dim3(256), args, smem, stream));
     return true;
@@ -1484,7 +1484,8 @@ bool launch_filter_project_tma(int64_t n_rows, const void* pred_in, int n_fixed_
     ARK_CUDA(cudaFuncSetAttribute(filter_project_tma_kernel<2, true, 512>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
     configured = true;
   }
-  KernelTimer t("filter_project_tma_kernel", stream);
+  if (n_fixed_out == 0 && !v) return false;  // before the timer: a declined launch is not recorded
+  KernelTimer t("filter_project_tma_kernel", stream, "filter_project_r1_kernel");
 #define ARK_TMA_LAUNCH(NF, V, TH) filter_project_tma_kernel<NF, V, TH><<<P.n_tiles, TH, (V) ? smem : 0, stream>>>(P)
   if (g_fp_threads == 256) {
     if (n_fixed_out == 0 && v) ARK_TMA_LAUNCH(0, true, 256);
