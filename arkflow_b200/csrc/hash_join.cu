@@ -13,6 +13,7 @@
 // build-side index is NO_ROW, which the gathers turn into NULLs (validity bitmaps on every build-side column).
 #include <cub/device/device_scan.cuh>
 
+#include "agg_acc.cuh"
 #include "engine.h"
 #include "hashkey.cuh"
 #include "stage_store.cuh"
@@ -119,15 +120,15 @@ __global__ void take_matched_kernel(const unsigned int* idx, long long n, uint8_
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) out_bytes[i] = idx[i] != NO_ROW;
 }
-__global__ void sum_lengths_kernel(const int32_t* lens, long long n, unsigned long long* total) {
-  unsigned long long acc = 0;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) acc += (unsigned long long)lens[i];
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-  if ((threadIdx.x & 31) == 0 && acc) atomicAdd(total, acc);
-}
-__global__ void take_lengths_kernel(const int32_t* offsets, const unsigned int* idx, long long n, int32_t* lens) {
+// The output offsets come from an int32 scan, which wraps silently once the bytes pass 2 GiB (and may wrap past 2^32
+// back to a positive total).  The kernels that write the lengths therefore also add them up in 64 bits: one atomicAdd
+// per warp into *total, which the host checks before it sizes the output.
+__global__ void take_lengths_kernel(const int32_t* offsets, const unsigned int* idx, long long n, int32_t* lens, unsigned long long* total) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) { const unsigned int r = idx[i]; lens[i] = r == NO_ROW ? 0 : offsets[r + 1] - offsets[r]; }
+  int32_t l = 0;
+  if (i < n) { const unsigned int r = idx[i]; l = r == NO_ROW ? 0 : offsets[r + 1] - offsets[r]; lens[i] = l; }
+  const long long s = warp_sum_ll(l);
+  if ((threadIdx.x & 31) == 0 && s) atomicAdd(total, (unsigned long long)s);
 }
 // All plain gathers of one output batch in ONE launch: every output row reads its (up to two) source row indices once,
 // then copies the 8-byte value of every fixed-width column and records the length of every string column.  One launch per
@@ -142,9 +143,14 @@ struct TakeMultiParams {
   uint8_t fside[TAKE_MAX_FIXED];
   const int32_t* soff[TAKE_MAX_STR];
   int32_t* slen[TAKE_MAX_STR];
+  unsigned long long* stotal;  // n_str words: each string column's 64-bit byte total (zeroed by the host)
   uint8_t sside[TAKE_MAX_STR];
 };
-__global__ void __launch_bounds__(256) take_multi_kernel(const __grid_constant__ TakeMultiParams P, long long n) {
+// 5 CTAs per SM (48 registers, no spills): without the bound ptxas spends 74 registers on the string totals, 3 CTAs per SM
+__global__ void __launch_bounds__(256, 5) take_multi_kernel(const __grid_constant__ TakeMultiParams P, long long n) {
+  // a thread's bytes per column, saturated at 2^31 (no wrap in 32 bits): exact while the column's total fits int32, and
+  // above 2^31 - 1 whenever the total does not
+  unsigned tot[TAKE_MAX_STR] = {0, 0, 0, 0};
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     unsigned int r[2];
     r[0] = P.idx[0] ? P.idx[0][i] : NO_ROW;
@@ -160,8 +166,14 @@ __global__ void __launch_bounds__(256) take_multi_kernel(const __grid_constant__
 #pragma unroll
     for (int c = 0; c < TAKE_MAX_FIXED; ++c) if (c < P.n_fixed) P.fdst[c][i] = v[c];
 #pragma unroll
-    for (int c = 0; c < TAKE_MAX_STR; ++c) if (c < P.n_str) P.slen[c][i] = l[c];
+    for (int c = 0; c < TAKE_MAX_STR; ++c) if (c < P.n_str) { P.slen[c][i] = l[c]; tot[c] = min(tot[c] + (unsigned)l[c], 0x80000000u); }
   }
+#pragma unroll
+  for (int c = 0; c < TAKE_MAX_STR; ++c)
+    if (c < P.n_str) {  // n_str is uniform: every lane of the warp takes part in the reduction
+      const long long s = warp_sum_ll((long long)tot[c]);
+      if ((threadIdx.x & 31) == 0 && s) atomicAdd(P.stotal + c, (unsigned long long)s);
+    }
 }
 // global → shared copy of one string, word-granular on the (shared) destination: aligned source words are
 // funnel-shifted into place, so a 12-byte key costs 3–4 loads and 3 stores instead of 12 + 12.
@@ -204,7 +216,7 @@ __global__ void __launch_bounds__(256) take_bytes_tile_kernel(const uint8_t* dat
   const int tid = threadIdx.x;
   const int32_t bb = out_offsets[row0];
   const int tb = out_offsets[row0 + rows] - bb;
-  if (tb + 16 > stage_bytes) {  // long strings: straight per-row copies, a warp per row
+  if (tb > stage_bytes - 16) {  // long strings: straight per-row copies, a warp per row (tb + 16 would overflow near 2 GiB)
     const int lane = tid & 31;
     for (int i = tid >> 5; i < rows; i += 8) {
       const unsigned int r = idx[row0 + i];
@@ -318,31 +330,22 @@ Column take_column(const Column& src, const unsigned int* idx, int64_t n, const 
       break;
     }
     case DType::Utf8: case DType::Binary: {
-      BufferPtr lens = device_alloc((size_t)(n + 1) * 4), offs = device_alloc((size_t)(n + 1) * 4);
-      ARK_CUDA(cudaMemsetAsync(lens.get(), 0, (size_t)(n + 1) * 4, stream));
-      if (n) { KernelTimer t("take_lengths_kernel", stream); take_lengths_kernel<<<g, 256, 0, stream>>>(src.offsets, idx, n, (int32_t*)lens.get()); }
-      {
-        // the int32 scan below wraps silently past 2 GiB: when the gathered bytes could get near that, add them up in 64 bits first
-        const double avg_len = src.length > 0 && src.data_bytes >= 0 ? (double)src.data_bytes / (double)src.length : 64.0;
-        if (avg_len * (double)n > 1.0e9) {
-          BufferPtr sum = device_alloc(16), hs = pinned_alloc(16);
-          ARK_CUDA(cudaMemsetAsync(sum.get(), 0, 16, stream));
-          { KernelTimer t("sum_lengths_kernel", stream); sum_lengths_kernel<<<(unsigned)std::min<int64_t>(ceil_div(n, 256), sm_count() * 16), 256, 0, stream>>>((const int32_t*)lens.get(), n, (unsigned long long*)sum.get()); }
-          ARK_CUDA(cudaMemcpyAsync(hs.get(), sum.get(), 8, cudaMemcpyDeviceToHost, stream));
-          ARK_CUDA(cudaStreamSynchronize(stream));
-          if (*(unsigned long long*)hs.get() > 2147483647ull) fail(ARK_ERR_PROCESS, "Collection query results error: Arrow error: offset overflow, result column exceeds 2 GiB");
-        }
-      }
+      // lens[n] = 0 closes the scan; the 64-bit total sits in the 8 bytes after it
+      BufferPtr lens = device_alloc((size_t)(n + 1) * 4 + 16), offs = device_alloc((size_t)(n + 1) * 4);
+      ARK_CUDA(cudaMemsetAsync(lens.get(), 0, (size_t)(n + 1) * 4 + 16, stream));
+      unsigned long long* total64 = (unsigned long long*)((uint8_t*)lens.get() + round_up((int64_t)(n + 1) * 4, 8));
+      if (n) { KernelTimer t("take_lengths_kernel", stream); take_lengths_kernel<<<g, 256, 0, stream>>>(src.offsets, idx, n, (int32_t*)lens.get(), total64); }
       size_t tb = 0;
       cub::DeviceScan::ExclusiveSum(nullptr, tb, (int32_t*)lens.get(), (int32_t*)offs.get(), (int)(n + 1), stream);
       BufferPtr tmp = device_alloc(tb + 16);
       note_launch("cub::DeviceScan::ExclusiveSum");
       cub::DeviceScan::ExclusiveSum(tmp.get(), tb, (int32_t*)lens.get(), (int32_t*)offs.get(), (int)(n + 1), stream);
       BufferPtr h = pinned_alloc(64);
-      ARK_CUDA(cudaMemcpyAsync(h.get(), (int32_t*)offs.get() + n, 4, cudaMemcpyDeviceToHost, stream));
+      ARK_CUDA(cudaMemcpyAsync(h.get(), total64, 8, cudaMemcpyDeviceToHost, stream));
       ARK_CUDA(cudaStreamSynchronize(stream));
-      const int32_t total = *(int32_t*)h.get();
-      if (total < 0) fail(ARK_ERR_PROCESS, "Collection query results error: Arrow error: offset overflow, result column exceeds 2 GiB");
+      const unsigned long long total64_h = *(const unsigned long long*)h.get();
+      if (total64_h > 2147483647ull) fail(ARK_ERR_PROCESS, "Collection query results error: Arrow error: offset overflow, result column exceeds 2 GiB");
+      const int32_t total = (int32_t)total64_h;  // = offs[n]: the scan did not wrap
       BufferPtr bytes = device_alloc((size_t)total + 16);
       if (n) {
         KernelTimer t("take_bytes_tile_kernel", stream);
@@ -390,6 +393,10 @@ std::vector<Column> take_columns(const std::vector<TakeSpec>& specs, const unsig
   memset(&P, 0, sizeof P);
   P.idx[0] = idx0; P.idx[1] = idx1;
   std::vector<BufferPtr> fbuf, lens, offs;
+  // each string column's 64-bit byte total: added up by take_multi_kernel, fetched in one round trip
+  BufferPtr sums = device_alloc(8 * (size_t)std::max<size_t>(strs.size(), 1)), h = pinned_alloc(8 * (size_t)std::max<size_t>(strs.size(), 1));
+  if (!strs.empty()) ARK_CUDA(cudaMemsetAsync(sums.get(), 0, 8 * strs.size(), stream));
+  P.stotal = (unsigned long long*)sums.get();
   for (int k : fixed) {
     BufferPtr d = device_alloc((size_t)n * 8);
     P.fsrc[P.n_fixed] = (const unsigned long long*)specs[k].src->data; P.fdst[P.n_fixed] = (unsigned long long*)d.get(); P.fside[P.n_fixed] = (uint8_t)specs[k].side;
@@ -405,35 +412,20 @@ std::vector<Column> take_columns(const std::vector<TakeSpec>& specs, const unsig
     KernelTimer t("take_multi_kernel", stream);
     take_multi_kernel<<<grid_for(n), 256, 0, stream>>>(P, n);
   }
-  // string columns: offsets by scan; every column's total (and, near 2 GiB, its 64-bit sum) comes back in one round trip
-  BufferPtr sums = device_alloc(8 * (size_t)std::max<size_t>(strs.size(), 1)), h = pinned_alloc(16 * (size_t)std::max<size_t>(strs.size(), 1));
-  bool check64 = false;
-  for (size_t j = 0; j < strs.size(); ++j) {
-    const Column& src = *specs[strs[j]].src;
-    const double avg_len = src.length > 0 && src.data_bytes >= 0 ? (double)src.data_bytes / (double)src.length : 64.0;
-    if (avg_len * (double)n > 1.0e9) check64 = true;
-  }
-  if (check64) {
-    ARK_CUDA(cudaMemsetAsync(sums.get(), 0, 8 * strs.size(), stream));
-    for (size_t j = 0; j < strs.size(); ++j) {
-      KernelTimer t("sum_lengths_kernel", stream);
-      sum_lengths_kernel<<<(unsigned)std::min<int64_t>(ceil_div(n, 256), sm_count() * 16), 256, 0, stream>>>((const int32_t*)lens[j].get(), n, (unsigned long long*)sums.get() + j);
-    }
-    ARK_CUDA(cudaMemcpyAsync((uint8_t*)h.get() + 8 * strs.size(), sums.get(), 8 * strs.size(), cudaMemcpyDeviceToHost, stream));
-  }
+  // string columns: offsets by scan; every column's total comes back in one round trip
+  if (!strs.empty()) ARK_CUDA(cudaMemcpyAsync(h.get(), sums.get(), 8 * strs.size(), cudaMemcpyDeviceToHost, stream));
   for (size_t j = 0; j < strs.size(); ++j) {
     size_t tb = 0;
     cub::DeviceScan::ExclusiveSum(nullptr, tb, (int32_t*)lens[j].get(), (int32_t*)offs[j].get(), (int)(n + 1), stream);
     BufferPtr tmp = device_alloc(tb + 16);
     note_launch("cub::DeviceScan::ExclusiveSum");
     cub::DeviceScan::ExclusiveSum(tmp.get(), tb, (int32_t*)lens[j].get(), (int32_t*)offs[j].get(), (int)(n + 1), stream);
-    ARK_CUDA(cudaMemcpyAsync((int32_t*)h.get() + j, (int32_t*)offs[j].get() + n, 4, cudaMemcpyDeviceToHost, stream));
   }
   if (!strs.empty()) ARK_CUDA(cudaStreamSynchronize(stream));
   for (size_t j = 0; j < strs.size(); ++j) {
-    const int32_t total = ((const int32_t*)h.get())[j];
-    const unsigned long long s64 = check64 ? ((const unsigned long long*)((const uint8_t*)h.get() + 8 * strs.size()))[j] : 0;
-    if (total < 0 || s64 > 2147483647ull) fail(ARK_ERR_PROCESS, "Collection query results error: Arrow error: offset overflow, result column exceeds 2 GiB");
+    const unsigned long long total64 = ((const unsigned long long*)h.get())[j];
+    if (total64 > 2147483647ull) fail(ARK_ERR_PROCESS, "Collection query results error: Arrow error: offset overflow, result column exceeds 2 GiB");
+    const int32_t total = (int32_t)total64;  // = offs[j][n]: the scan did not wrap
     const TakeSpec& sp = specs[strs[j]];
     BufferPtr bytes = device_alloc((size_t)total + 16);
     {

@@ -7,6 +7,7 @@
 // lengths → exclusive scan → one thread per row writes its parts.
 #include <cub/device/device_scan.cuh>
 
+#include "agg_acc.cuh"
 #include "engine.h"
 #include "stage_store.cuh"
 
@@ -65,14 +66,19 @@ __device__ __forceinline__ int part_len(const ConcatPartView& p, int64_t r, cons
   return p.offsets[r + 1] - o0;
 }
 
-__global__ void concat_lengths_kernel(const __grid_constant__ ConcatParams P, int32_t* lens) {
+// lens[r] = bytes of row r; *sum += all of them in 64 bits (the int32 scan of lens wraps silently past 2 GiB, and a
+// literal repeated on every row can take the total past 2^32 back to a positive int32)
+__global__ void concat_lengths_kernel(const __grid_constant__ ConcatParams P, int32_t* lens, unsigned long long* sum) {
   const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= P.n_rows) return;
   int total = 0;
-  const uint8_t* src;
-  uint8_t scratch[24];
-  for (int k = 0; k < P.n_parts; ++k) total += part_len(P.parts[k], r, &src, scratch);
-  lens[r] = total;
+  if (r < P.n_rows) {
+    const uint8_t* src;
+    uint8_t scratch[24];
+    for (int k = 0; k < P.n_parts; ++k) total += part_len(P.parts[k], r, &src, scratch);
+    lens[r] = total;
+  }
+  const long long s = warp_sum_ll(total);
+  if ((threadIdx.x & 31) == 0 && s) atomicAdd(sum, (unsigned long long)s);
 }
 
 __device__ __forceinline__ void concat_row(const ConcatParams& P, int64_t r, uint8_t* d) {
@@ -95,7 +101,7 @@ __global__ void __launch_bounds__(CONCAT_THREADS) concat_write_kernel(const __gr
   const int64_t r = r0 + threadIdx.x;
   const int32_t bb = out_offsets[r0];
   const int tb = out_offsets[r0 + rows] - bb;
-  if (tb + 16 > stage_bytes) {
+  if (tb > stage_bytes - 16) {  // (tb + 16 would overflow near 2 GiB)
     if (r < P.n_rows) concat_row(P, r, out + out_offsets[r]);
     return;
   }
@@ -109,20 +115,24 @@ __global__ void __launch_bounds__(CONCAT_THREADS) concat_write_kernel(const __gr
 
 // lengths → scan → bytes for one string column described by P; returns the offsets / bytes of the n_rows strings
 static void render_strings(const ConcatParams& P, int64_t n, cudaStream_t stream, BufferPtr* out_offs, BufferPtr* out_bytes, int32_t* out_total) {
-  BufferPtr lens = device_alloc((size_t)(n + 1) * 4), offs = device_alloc((size_t)(n + 1) * 4);
-  ARK_CUDA(cudaMemsetAsync((int32_t*)lens.get() + n, 0, 4, stream));
+  // lens[n] = 0 closes the scan; the 64-bit total sits in the 8 bytes after it
+  BufferPtr lens = device_alloc((size_t)(n + 1) * 4 + 16), offs = device_alloc((size_t)(n + 1) * 4);
+  const int64_t sum_at = round_up((int64_t)(n + 1) * 4, 8);
+  ARK_CUDA(cudaMemsetAsync((int32_t*)lens.get() + n, 0, (size_t)(sum_at + 8 - n * 4), stream));
+  unsigned long long* sum = (unsigned long long*)((uint8_t*)lens.get() + sum_at);
   const unsigned grid = (unsigned)std::max<int64_t>(1, ceil_div(n, 256));
-  if (n) { KernelTimer t("concat_lengths_kernel", stream); concat_lengths_kernel<<<grid, 256, 0, stream>>>(P, (int32_t*)lens.get()); }
+  if (n) { KernelTimer t("concat_lengths_kernel", stream); concat_lengths_kernel<<<grid, 256, 0, stream>>>(P, (int32_t*)lens.get(), sum); }
   size_t tb = 0;
   cub::DeviceScan::ExclusiveSum(nullptr, tb, (int32_t*)lens.get(), (int32_t*)offs.get(), (int)(n + 1), stream);
   BufferPtr tmp = device_alloc(tb + 16);
   note_launch("cub::DeviceScan::ExclusiveSum");
   cub::DeviceScan::ExclusiveSum(tmp.get(), tb, (int32_t*)lens.get(), (int32_t*)offs.get(), (int)(n + 1), stream);
   BufferPtr h = pinned_alloc(64);
-  ARK_CUDA(cudaMemcpyAsync(h.get(), (int32_t*)offs.get() + n, 4, cudaMemcpyDeviceToHost, stream));
+  ARK_CUDA(cudaMemcpyAsync(h.get(), sum, 8, cudaMemcpyDeviceToHost, stream));
   ARK_CUDA(cudaStreamSynchronize(stream));
-  const int32_t total = *(const int32_t*)h.get();
-  if (total < 0) fail(ARK_ERR_PROCESS, "Collection query results error: Arrow error: offset overflow, string result exceeds 2 GiB");
+  const unsigned long long total64 = *(const unsigned long long*)h.get();
+  if (total64 > 2147483647ull) fail(ARK_ERR_PROCESS, "Collection query results error: Arrow error: offset overflow, string result exceeds 2 GiB");
+  const int32_t total = (int32_t)total64;  // = offs[n]: the scan did not wrap
   BufferPtr bytes = device_alloc((size_t)total + 16);
   if (n) {
     const int stage = (int)std::min<int64_t>(44 * 1024, round_up((int64_t)((double)total / (double)n * CONCAT_THREADS * 1.5) + 256, 1024));
