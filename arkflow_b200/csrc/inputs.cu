@@ -32,6 +32,7 @@
 #include "decimal.cuh"
 #include "engine.h"
 #include "json_mini.h"
+#include "utf8.cuh"
 
 using namespace ark;
 
@@ -119,7 +120,7 @@ struct CsvParams {
   int32_t* str_len[CSV_MAX_COLS];    // Utf8: decoded length per row (n_rows + 1 entries; scanned into offsets)
   long long* str_src[CSV_MAX_COLS];  // Utf8: absolute position of the field body
   int32_t* str_raw[CSV_MAX_COLS];    // Utf8: raw length; negative ⇒ quoted field with "" escapes
-  int32_t* error;                    // [0] = 1 bad number / 2 wrong field count, [1] = row
+  int32_t* error;                    // [0] = 1 bad number / 2 wrong field count / 3 invalid UTF-8 in a Utf8 field, [1] = row
 };
 
 // The host's type inference (csv_infer_type) calls the same two grammar tests as the kernel, so a column inferred
@@ -169,7 +170,7 @@ __global__ void csv_parse_kernel(const __grid_constant__ CsvParams P) {
     long long pos = P.line_off[row], end = P.line_off[row + 1];
     while (end > pos && (P.data[end - 1] == '\n' || P.data[end - 1] == '\r')) --end;
     int col = 0;
-    bool bad = false;
+    bool bad = false, bad_utf8 = false;
     while (col < P.n_cols) {
       long long f0 = pos, f1;
       bool escaped = false;
@@ -209,6 +210,7 @@ __global__ void csv_parse_kernel(const __grid_constant__ CsvParams P) {
           P.str_src[col][row] = f0;
           P.str_raw[col][row] = escaped ? -len : len;
           // arrow-csv: an empty unquoted field of a Utf8 column is NULL too (nulls are decided before the type)
+          if (!utf8_valid(fp, len)) bad_utf8 = true;  // a Utf8 array holds valid UTF-8 ("" escapes are ASCII)
           break;
         }
       }
@@ -218,6 +220,7 @@ __global__ void csv_parse_kernel(const __grid_constant__ CsvParams P) {
     }
     if (!bad && pos < end) { bad = true; if (atomicCAS(P.error, 0, 2) == 0) P.error[1] = (int32_t)row; }  // more fields than the header
     else if (bad && atomicCAS(P.error, 0, 1) == 0) P.error[1] = (int32_t)row;
+    else if (bad_utf8 && atomicCAS(P.error, 0, 3) == 0) P.error[1] = (int32_t)row;
   }
 }
 
@@ -427,6 +430,9 @@ void csv_prepare(ark_input* in, cudaStream_t stream) {
     return s;
   };
   std::vector<std::string> head = split_csv_line(line(0), (char)in->delim);
+  if (in->has_header)
+    for (auto& h : head)
+      if (!utf8_valid((const uint8_t*)h.data(), (long long)h.size())) fail(ARK_ERR_PROCESS, "Read input failed: Arrow error: Csv error: Encountered invalid UTF-8 data for line 1");
   if (in->has_header) in->csv_names = head;
   else for (size_t i = 0; i < head.size(); ++i) in->csv_names.push_back("column_" + std::to_string(i + 1));
   if ((int)in->csv_names.size() > CSV_MAX_COLS) fail(ARK_ERR_UNSUPPORTED, "csv input: more than 32 columns");
@@ -489,7 +495,8 @@ Batch csv_batch(ark_input* in, int64_t l0, int64_t n, cudaStream_t stream) {
   if (ecode) {
     const long long lineno = l0 + erow + 1;
     fail(ARK_ERR_PROCESS, ecode == 2 ? "Read input failed: Arrow error: Csv error: incorrect number of fields for line " + std::to_string(lineno)
-                                     : "Read input failed: Arrow error: Parser error: Error while parsing value of line " + std::to_string(lineno));
+                          : ecode == 3 ? "Read input failed: Arrow error: Csv error: Encountered invalid UTF-8 data for line " + std::to_string(lineno)
+                                       : "Read input failed: Arrow error: Parser error: Error while parsing value of line " + std::to_string(lineno));
   }
   Batch b;
   b.num_rows = n;

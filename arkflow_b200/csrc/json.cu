@@ -22,6 +22,7 @@
 #include "tma.cuh"
 #include "json_mini.h"
 #include "decimal.cuh"
+#include "utf8.cuh"
 
 namespace ark {
 
@@ -30,8 +31,10 @@ namespace {
 constexpr int JS_MAX_FIELDS = 16;   // fields that travel in the kernel parameter block (constant bank); larger schemas use a table in HBM
 constexpr int JS_MAX_NAME = 48;     // name bytes held inline; longer names are read through long_name
 constexpr int JS_MAX_FIELDS_EXT = 64;  // the per-record `seen` mask is 64 bits wide
+constexpr int JS_QUOTED_NUM_MAX = 128;  // decoded bytes of a quoted number written with escapes (parse_escaped_number)
 
-enum JsonErr : int32_t { JE_NONE = 0, JE_SYNTAX = 1, JE_NOT_OBJECT = 2, JE_TYPE = 3, JE_NUMBER = 4 };
+// JE_STRING: a string that is not well-formed (escape, surrogate pairing or raw UTF-8), see strings_valid
+enum JsonErr : int32_t { JE_NONE = 0, JE_SYNTAX = 1, JE_NOT_OBJECT = 2, JE_TYPE = 3, JE_NUMBER = 4, JE_STRING = 5 };
 
 struct JsonField {
   int32_t dtype;     // DType as int
@@ -61,7 +64,8 @@ struct JsonParams {
   const int32_t* span_len;
   const long long* row_start;  // pass A: first output row of payload i
   int32_t* counts;             // count pass: records in payload i
-  int32_t* error;              // [0] = JsonErr, [1] = payload index (first error wins), [2] = some payload does not hold exactly one record
+  int32_t* error;              // [0] = JsonErr, [1] = payload index (first error wins), [2] = some payload does not hold exactly one record,
+                               // [3] = some Int64 / Float64 row is a quoted number with escapes (valid_bytes 2, see json_quoted_numbers_kernel)
   int32_t stage_bytes;         // shared-memory staging window per CTA (0 = parse straight from global memory)
 };
 
@@ -71,6 +75,7 @@ constexpr int JS_THREADS = 128;
 struct Cursor {
   const uint8_t* p;
   const uint8_t* end;
+  unsigned need = 0;  // bit 7: some string skip_string passed holds an escape or a byte >= 0x80 (see strings_valid)
 };
 
 __device__ __forceinline__ bool is_ws(unsigned ch) {  // ' ' \t \n \r: one range test + one bit test
@@ -80,20 +85,87 @@ __device__ __forceinline__ void skip_ws(Cursor& c) {
   while (c.p < c.end && is_ws(*c.p)) ++c.p;
 }
 
-// cursor on the opening quote; leaves it after the closing quote. Returns false on a malformed string.
+__device__ __forceinline__ unsigned hex_digit(unsigned h) {  // 16 when h is not a hex digit
+  const unsigned l = h | 0x20;
+  return h - '0' <= 9u ? h - '0' : l - 'a' <= 5u ? l - 'a' + 10 : 16;
+}
+
+// The escape at p (on its backslash) must be one of JSON's nine; \u takes four hex digits, a high surrogate must be
+// followed by a \u low surrogate, and a low surrogate may not stand alone.  Returns the position after the escape,
+// nullptr when it is malformed.
+__device__ __forceinline__ const uint8_t* skip_escape(const uint8_t* p, const uint8_t* end) {
+  if (end - p < 2) return nullptr;
+  const uint8_t e = p[1];
+  if (e != 'u') return e == '"' || e == '\\' || e == '/' || e == 'b' || e == 'f' || e == 'n' || e == 'r' || e == 't' ? p + 2 : nullptr;
+  auto hex4 = [&](const uint8_t* q, unsigned* cp) {
+    if (end - q < 4) return false;
+    unsigned v = 0;
+    for (int k = 0; k < 4; ++k) { const unsigned d = hex_digit(q[k]); if (d > 15) return false; v = v * 16 + d; }
+    *cp = v;
+    return true;
+  };
+  unsigned hi, lo;
+  if (!hex4(p + 2, &hi)) return nullptr;
+  p += 6;
+  if (hi < 0xD800 || hi > 0xDFFF) return p;
+  if (hi >= 0xDC00) return nullptr;  // a low surrogate with no high one before it
+  if (end - p < 2 || p[0] != '\\' || p[1] != 'u' || !hex4(p + 2, &lo) || lo < 0xDC00 || lo > 0xDFFF) return nullptr;
+  return p + 6;
+}
+
+// Is the string body b[0..len) well-formed: every escape accepted by skip_escape, the raw bytes well-formed UTF-8 (an
+// arrow-rs StringArray always holds valid UTF-8)?
+__device__ __noinline__ bool body_valid(const uint8_t* b, int len) {
+  const uint8_t* end = b + len;
+  for (const uint8_t* p = b; p < end;) {
+    if (*p != '\\') { ++p; continue; }
+    p = skip_escape(p, end);
+    if (!p) return false;
+  }
+  return utf8_valid(b, len);
+}
+
+// Cursor on the opening quote; leaves it after the closing quote.  Returns false when the string is unterminated or
+// holds a raw control byte.  Every string the decoder reads passes through here — keys, values, skipped values and
+// the spans the List / Struct stages decode again.  The scan is the plain one (an escape skips the byte after the
+// backslash) and costs ASCII text nothing more: the common branch takes bytes above '\\' as signed chars, so a byte
+// >= 0x80 falls through to the rarer branches, where it is noted like an escape.  A string with either sets bit 7 of
+// c.need, and json_parse_kernel then checks that payload's strings once (strings_valid), out of line.
 __device__ bool skip_string(Cursor& c, const uint8_t** body, int* raw_len, bool* has_escape) {
   ++c.p;
   const uint8_t* start = c.p;
   bool esc = false;
+  unsigned other = 0;  // OR of the bytes off the common branch: bit 7 set <=> a byte >= 0x80
   while (c.p < c.end) {
     const uint8_t ch = *c.p;
-    if (ch > '\\') { ++c.p; continue; }  // lower-case letters, '_', '{', UTF-8 continuation bytes: the common case first
-    if (ch == '"') { *body = start; *raw_len = (int)(c.p - start); *has_escape = esc; ++c.p; return true; }
+    if ((int8_t)ch > '\\') { ++c.p; continue; }  // lower-case letters, '_', '{': the common case first
+    if (ch == '"') {
+      c.need |= other | (esc ? 0x80u : 0u);
+      *body = start; *raw_len = (int)(c.p - start); *has_escape = esc; ++c.p;
+      return true;
+    }
     if (ch == '\\') { esc = true; c.p += 2; continue; }
     if (ch < 0x20) return false;
+    other |= ch;
     ++c.p;
   }
   return false;
+}
+
+// Are the strings of the payload b[0..end) well-formed (body_valid)?  Called once per payload whose strings set bit 7
+// of Cursor::need, after the payload parsed: its strings are terminated and nothing outside them is a quote or a byte
+// >= 0x80.  A malformed string is JE_STRING wherever it stands — key, value, skipped value, inside a List or Struct
+// span — so the List / Struct stages and json_strings_kernel only ever see well-formed bodies.
+__device__ __noinline__ bool strings_valid(const uint8_t* b, const uint8_t* end) {
+  while (b < end) {
+    if (*b++ != '"') continue;
+    const uint8_t* s = b;
+    while (b < end && *b != '"') b += *b == '\\' ? 2 : 1;
+    if (b > end) b = end;
+    if (!body_valid(s, (int)(b - s))) return false;
+    ++b;
+  }
+  return true;
 }
 
 __device__ bool skip_value(Cursor& c, int depth);
@@ -189,70 +261,52 @@ __device__ bool parse_i64(const uint8_t* s, int len, long long* out) {
   return true;
 }
 
-// length of a JSON string body once escapes are decoded; -1 if malformed
+// Decoding.  json_strings_kernel, the List stage and json_quoted_numbers_kernel decode bodies that strings_valid has
+// accepted; the parse kernels measure and compare bodies before their payload is checked, so the escape reader stays
+// inside b[0..raw) whatever it holds (a malformed body then fails the payload's check).
+__device__ __forceinline__ unsigned hex4_unchecked(const uint8_t* q) {
+  unsigned v = 0;
+  for (int k = 0; k < 4; ++k) v = v * 16 + hex_digit(q[k]);
+  return v;
+}
+
+// the escape at b[*i] (on its backslash) of the body b[0..raw) → its code point, a surrogate pair combined; *i moves past it
+__device__ __forceinline__ unsigned escape_cp(const uint8_t* b, int raw, int* i) {
+  const uint8_t e = *i + 1 < raw ? b[*i + 1] : '\\';
+  if (e != 'u' || *i + 6 > raw) { *i += 2; return e == 'b' ? '\b' : e == 'f' ? '\f' : e == 'n' ? '\n' : e == 'r' ? '\r' : e == 't' ? '\t' : e; }
+  unsigned cp = hex4_unchecked(b + *i + 2);
+  *i += 6;
+  if (cp >= 0xD800 && cp < 0xDC00 && *i + 6 <= raw) { cp = 0x10000 + ((cp - 0xD800) << 10) + (hex4_unchecked(b + *i + 2) - 0xDC00); *i += 6; }
+  return cp;
+}
+
+__device__ __forceinline__ int put_utf8(unsigned cp, uint8_t* out) {
+  if (cp < 0x80) { out[0] = (uint8_t)cp; return 1; }
+  if (cp < 0x800) { out[0] = 0xC0 | (cp >> 6); out[1] = 0x80 | (cp & 0x3F); return 2; }
+  if (cp < 0x10000) { out[0] = 0xE0 | (cp >> 12); out[1] = 0x80 | ((cp >> 6) & 0x3F); out[2] = 0x80 | (cp & 0x3F); return 3; }
+  out[0] = 0xF0 | (cp >> 18); out[1] = 0x80 | ((cp >> 12) & 0x3F); out[2] = 0x80 | ((cp >> 6) & 0x3F); out[3] = 0x80 | (cp & 0x3F);
+  return 4;
+}
+
+// length of a JSON string body once escapes are decoded
 __device__ int decoded_len(const uint8_t* b, int raw) {
   int n = 0;
   for (int i = 0; i < raw;) {
     if (b[i] != '\\') { ++n; ++i; continue; }
-    if (i + 1 >= raw) return -1;
-    const uint8_t e = b[i + 1];
-    if (e == 'u') {
-      if (i + 6 > raw) return -1;
-      unsigned cp = 0;
-      for (int k = 2; k < 6; ++k) {
-        const uint8_t h = b[i + k];
-        unsigned d = h >= '0' && h <= '9' ? h - '0' : h >= 'a' && h <= 'f' ? h - 'a' + 10 : h >= 'A' && h <= 'F' ? h - 'A' + 10 : 99;
-        if (d == 99) return -1;
-        cp = cp * 16 + d;
-      }
-      i += 6;
-      if (cp >= 0xD800 && cp < 0xDC00) {  // high surrogate: needs \uDC00..DFFF
-        if (i + 6 > raw || b[i] != '\\' || b[i + 1] != 'u') return -1;
-        i += 6;
-        n += 4;
-      } else n += cp < 0x80 ? 1 : cp < 0x800 ? 2 : 3;
-    } else {
-      if (e != '"' && e != '\\' && e != '/' && e != 'b' && e != 'f' && e != 'n' && e != 'r' && e != 't') return -1;
-      ++n; i += 2;
-    }
+    const unsigned cp = escape_cp(b, raw, &i);
+    n += cp < 0x80 ? 1 : cp < 0x800 ? 2 : cp < 0x10000 ? 3 : 4;
   }
   return n;
 }
 
-// does the JSON string body b[0..raw) (which contains escapes) decode to exactly nm[0..nlen)?  Malformed escapes: no.
+// does the JSON string body b[0..raw) (which contains escapes) decode to exactly nm[0..nlen)?
 __device__ bool decoded_equals(const uint8_t* b, int raw, const char* nm, int nlen) {
   int n = 0;
   for (int i = 0; i < raw;) {
     uint8_t out[4];
-    int k = 0;
-    if (b[i] != '\\') { out[k++] = b[i++]; }
-    else {
-      if (i + 1 >= raw) return false;
-      const uint8_t e = b[i + 1];
-      if (e == 'u') {
-        if (i + 6 > raw) return false;
-        auto hex4 = [&](int at, unsigned* cp) { unsigned v = 0; for (int q = 0; q < 4; ++q) { const uint8_t h = b[at + q];
-          const unsigned d = h >= '0' && h <= '9' ? h - '0' : h >= 'a' && h <= 'f' ? h - 'a' + 10 : h >= 'A' && h <= 'F' ? h - 'A' + 10 : 99; if (d == 99) return false; v = v * 16 + d; } *cp = v; return true; };
-        unsigned cp;
-        if (!hex4(i + 2, &cp)) return false;
-        i += 6;
-        if (cp >= 0xD800 && cp < 0xDC00) {
-          unsigned lo;
-          if (i + 6 > raw || b[i] != '\\' || b[i + 1] != 'u' || !hex4(i + 2, &lo)) return false;
-          i += 6;
-          cp = 0x10000 + ((cp - 0xD800) << 10) + (lo - 0xDC00);
-        }
-        if (cp < 0x80) out[k++] = (uint8_t)cp;
-        else if (cp < 0x800) { out[k++] = 0xC0 | (cp >> 6); out[k++] = 0x80 | (cp & 0x3F); }
-        else if (cp < 0x10000) { out[k++] = 0xE0 | (cp >> 12); out[k++] = 0x80 | ((cp >> 6) & 0x3F); out[k++] = 0x80 | (cp & 0x3F); }
-        else { out[k++] = 0xF0 | (cp >> 18); out[k++] = 0x80 | ((cp >> 12) & 0x3F); out[k++] = 0x80 | ((cp >> 6) & 0x3F); out[k++] = 0x80 | (cp & 0x3F); }
-      } else {
-        uint8_t ch = e;
-        if (e == 'b') ch = '\b'; else if (e == 'f') ch = '\f'; else if (e == 'n') ch = '\n'; else if (e == 'r') ch = '\r'; else if (e == 't') ch = '\t';
-        else if (e != '"' && e != '\\' && e != '/') return false;
-        out[k++] = ch; i += 2;
-      }
-    }
+    int k = 1;
+    if (b[i] != '\\') out[0] = b[i++];
+    else k = put_utf8(escape_cp(b, raw, &i), out);
     for (int q = 0; q < k; ++q) { if (n >= nlen || (uint8_t)nm[n] != out[q]) return false; ++n; }
   }
   return n == nlen;
@@ -261,22 +315,19 @@ __device__ bool decoded_equals(const uint8_t* b, int raw, const char* nm, int nl
 __device__ void decode_string(const uint8_t* b, int raw, uint8_t* out) {
   for (int i = 0; i < raw;) {
     if (b[i] != '\\') { *out++ = b[i++]; continue; }
-    const uint8_t e = b[i + 1];
-    if (e == 'u') {
-      auto hex4 = [&](int at) { unsigned cp = 0; for (int k = 0; k < 4; ++k) { const uint8_t h = b[at + k]; cp = cp * 16 + (h <= '9' ? h - '0' : (h | 0x20) - 'a' + 10); } return cp; };
-      unsigned cp = hex4(i + 2);
-      i += 6;
-      if (cp >= 0xD800 && cp < 0xDC00) { const unsigned lo = hex4(i + 2); i += 6; cp = 0x10000 + ((cp - 0xD800) << 10) + (lo - 0xDC00); }
-      if (cp < 0x80) *out++ = (uint8_t)cp;
-      else if (cp < 0x800) { *out++ = 0xC0 | (cp >> 6); *out++ = 0x80 | (cp & 0x3F); }
-      else if (cp < 0x10000) { *out++ = 0xE0 | (cp >> 12); *out++ = 0x80 | ((cp >> 6) & 0x3F); *out++ = 0x80 | (cp & 0x3F); }
-      else { *out++ = 0xF0 | (cp >> 18); *out++ = 0x80 | ((cp >> 12) & 0x3F); *out++ = 0x80 | ((cp >> 6) & 0x3F); *out++ = 0x80 | (cp & 0x3F); }
-    } else {
-      uint8_t ch = e;
-      if (e == 'b') ch = '\b'; else if (e == 'f') ch = '\f'; else if (e == 'n') ch = '\n'; else if (e == 'r') ch = '\r'; else if (e == 't') ch = '\t';
-      *out++ = ch; i += 2;
-    }
+    out += put_utf8(escape_cp(b, raw, &i), out);
   }
+}
+
+// A quoted number written with escapes (a digit spelled as a u-escape): decoded, then parsed like any number body, as
+// arrow-json decodes the string first.  Out of line: a cold branch the parse kernels' registers do not carry.  A
+// decoded text longer than JS_QUOTED_NUM_MAX bytes is no number this decoder reads.
+__device__ __noinline__ bool parse_escaped_number(const uint8_t* b, int raw, bool as_i64, void* out) {
+  const int n = decoded_len(b, raw);
+  if (n > JS_QUOTED_NUM_MAX) return false;
+  uint8_t buf[JS_QUOTED_NUM_MAX];
+  decode_string(b, raw, buf);
+  return as_i64 ? parse_i64(buf, n, (long long*)out) : parse_f64(buf, n, (double*)out);
 }
 
 __device__ void raise(const JsonParams& P, int code, int64_t payload) {
@@ -291,8 +342,10 @@ __device__ void raise(const JsonParams& P, int code, int64_t payload) {
 // bulk copy (cp.async.bulk → mbarrier) of the 16-byte-aligned window around them and every thread parses
 // its payload from shared memory: 63-byte messages read byte by byte from global memory touch ~16 cache
 // lines per warp instruction; from shared memory an odd stride is conflict-free.
+// Nine CTAs per SM keep MODE 1 / 2 at 56 registers: left free, ptxas takes 64 and the SM holds one CTA fewer, which
+// made the parse ~12 % slower on 63-byte messages (H100).
 template <int MODE>
-__global__ void __launch_bounds__(JS_THREADS) json_parse_kernel(const __grid_constant__ JsonParams P) {
+__global__ void __launch_bounds__(JS_THREADS, 9) json_parse_kernel(const __grid_constant__ JsonParams P) {
   extern __shared__ __align__(16) uint8_t js_stage[];
   __shared__ __align__(8) unsigned long long s_bar;
   __shared__ long long s_stage_off;  // payload-column byte offset of js_stage[0] (may be slightly negative)
@@ -393,9 +446,16 @@ __global__ void __launch_bounds__(JS_THREADS) json_parse_kernel(const __grid_con
         case DType::Int64: case DType::Float64: {
           const uint8_t* ns; int nl;
           FastInt fi{false, 0};
-          if (ch == '"') { bool e; if (!skip_string(c, &ns, &nl, &e)) { raise(P, JE_SYNTAX, i); return; } }
+          bool nesc = false;
+          if (ch == '"') { if (!skip_string(c, &ns, &nl, &nesc)) { raise(P, JE_SYNTAX, i); return; } }
           else if (ch == '-' || (ch >= '0' && ch <= '9')) { if (!skip_number(c, &ns, &nl, &fi)) { raise(P, JE_SYNTAX, i); return; } }
           else { raise(P, JE_TYPE, i); return; }
+          if (nesc) {  // rare: json_quoted_numbers_kernel decodes and parses it, so this kernel carries no call for it
+            if (nl > 0xFFFF) { raise(P, JE_NUMBER, i); return; }  // decodes to far more than JS_QUOTED_NUM_MAX bytes
+            ((long long*)F.values)[row] = (long long)(ns - origin) << 16 | nl;
+            F.valid_bytes[row] = 2; seen |= 1ull << f; P.error[3] = 1;
+            continue;
+          }
           if ((DType)F.dtype == DType::Int64) {
             long long v = fi.value;
             if (!fi.ok && !parse_i64(ns, nl, &v)) { raise(P, JE_NUMBER, i); return; }
@@ -417,9 +477,7 @@ __global__ void __launch_bounds__(JS_THREADS) json_parse_kernel(const __grid_con
           if (ch != '"') { raise(P, JE_TYPE, i); return; }
           const uint8_t* sb; int sl; bool esc;
           if (!skip_string(c, &sb, &sl, &esc)) { raise(P, JE_SYNTAX, i); return; }
-          int dl = sl;
-          if (esc) { dl = decoded_len(sb, sl); if (dl < 0) { raise(P, JE_SYNTAX, i); return; } }
-          F.str_len[row] = dl; F.str_src[row] = (long long)(sb - origin); F.str_raw_len[row] = esc ? -sl : sl;
+          F.str_len[row] = esc ? decoded_len(sb, sl) : sl; F.str_src[row] = (long long)(sb - origin); F.str_raw_len[row] = esc ? -sl : sl;
           break;
         }
         case DType::List: case DType::Struct: {  // the raw span of the value; its elements / fields are decoded by a second stage
@@ -442,6 +500,10 @@ __global__ void __launch_bounds__(JS_THREADS) json_parse_kernel(const __grid_con
       }
     }
     ++row; ++records;
+  }
+  if (c.need & 0x80) {  // the payload's start is read again rather than kept in a register through the parse
+    const uint8_t* c0 = P.span_src ? P.data + P.span_src[i] : origin + P.offsets[i];
+    if (!strings_valid(c0, c.end)) { raise(P, JE_STRING, i); return; }
   }
   if (MODE == 0) P.counts[i] = records;
   if (MODE == 2 && records != 1) {
@@ -498,10 +560,13 @@ __global__ void json_list_fill_kernel(const uint8_t* data, const long long* src,
         case DType::Int64: case DType::Float64: {
           const uint8_t* ns; int nl;
           FastInt fi{false, 0};
-          if (ch == '"') { bool esc; if (!skip_string(c, &ns, &nl, &esc)) { bad(JE_SYNTAX); return; } }
+          bool nesc = false;
+          if (ch == '"') { if (!skip_string(c, &ns, &nl, &nesc)) { bad(JE_SYNTAX); return; } }
           else if (ch == '-' || (ch >= '0' && ch <= '9')) { if (!skip_number(c, &ns, &nl, &fi)) { bad(JE_SYNTAX); return; } }
           else { bad(JE_TYPE); return; }
-          if ((DType)elem_dtype == DType::Int64) {
+          if (nesc) {
+            if (!parse_escaped_number(ns, nl, (DType)elem_dtype == DType::Int64, (uint8_t*)values + e * 8)) { bad(JE_NUMBER); return; }
+          } else if ((DType)elem_dtype == DType::Int64) {
             long long v = fi.value;
             if (!fi.ok && !parse_i64(ns, nl, &v)) { bad(JE_NUMBER); return; }
             ((long long*)values)[e] = v;
@@ -522,9 +587,8 @@ __global__ void json_list_fill_kernel(const uint8_t* data, const long long* src,
           if (ch != '"') { bad(JE_TYPE); return; }
           const uint8_t* sb; int sl; bool esc;
           if (!skip_string(c, &sb, &sl, &esc)) { bad(JE_SYNTAX); return; }
-          int dl = sl;
-          if (esc) { dl = decoded_len(sb, sl); if (dl < 0) { bad(JE_SYNTAX); return; } }
-          str_len[e] = dl; str_src[e] = (long long)(sb - data); str_raw[e] = esc ? -sl : sl;
+          str_len[e] = esc ? decoded_len(sb, sl) : sl;  // the parse pass checked the span's strings
+          str_src[e] = (long long)(sb - data); str_raw[e] = esc ? -sl : sl;
           break;
         }
         default: bad(JE_TYPE); return;  // List<Null>: only nulls
@@ -535,6 +599,19 @@ __global__ void json_list_fill_kernel(const uint8_t* data, const long long* src,
     skip_ws(c);
     if (c.p < c.end && *c.p == ',') ++c.p;
   }
+}
+
+// Rows of one Int64 / Float64 column whose value was a quoted number with escapes: the parse kernel left valid_bytes 2
+// and values = (column byte offset of the body << 16 | raw length).  Decoded and parsed here; thread per row.
+__global__ void json_quoted_numbers_kernel(const uint8_t* data, int64_t n, bool as_i64, long long* values, uint8_t* valid, int32_t* error) {
+  const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n || valid[r] != 2) return;
+  const long long span = values[r];
+  if (!parse_escaped_number(data + (span >> 16), (int)(span & 0xFFFF), as_i64, values + r)) {
+    if (atomicCAS(error, 0, JE_NUMBER) == 0) error[1] = (int32_t)r;
+    return;
+  }
+  valid[r] = 1;
 }
 
 // string bytes of one Utf8 column: thread per row
@@ -630,6 +707,7 @@ std::vector<InferredField> infer_schema(const std::string& first_record) {
       else if (depth == 0 && !isspace((unsigned char)ch)) break;
     }
     if (end == std::string::npos) fail(ARK_ERR_PROCESS, "Schema inference error: Json error: Expected JSON record to be an object");
+    if (!utf8_valid((const uint8_t*)s.data(), (long long)end)) fail(ARK_ERR_PROCESS, "Schema inference error: Json error: invalid UTF-8");
     v = parse_json(s.substr(0, end));
   } catch (const ArkError& e) {
     if (e.code == ARK_ERR_SERIALIZATION) fail(ARK_ERR_PROCESS, std::string("Schema inference error: Json error: ") + e.what());
@@ -679,6 +757,7 @@ const char* json_err_text(int code) {
     case JE_NOT_OBJECT: return "Arrow JSON Reader Error: Json error: expected { got a non-object value";
     case JE_TYPE: return "Arrow JSON Reader Error: Json error: whilst decoding field: value does not match the inferred column type";
     case JE_NUMBER: return "Arrow JSON Reader Error: Json error: failed to parse number";
+    case JE_STRING: return "Arrow JSON Reader Error: Json error: invalid string: a malformed escape, an unpaired surrogate or invalid UTF-8";
     default: return "Arrow JSON Reader Error: Json error: Encountered unexpected token / truncated record";
   }
 }
@@ -919,6 +998,18 @@ bool decode_fields(const std::vector<InferredField>& specs, JsonParams Q, unsign
   const int32_t* e = (const int32_t*)h.get();
   if (optimistic && (e[0] != JE_NONE || e[2])) return false;
   if (e[0] != JE_NONE) raise_json(e[0], e[1], Q.span_src ? "row" : "payload");
+  if (e[3]) {  // quoted numbers written with escapes
+    ARK_CUDA(cudaMemsetAsync(err.get(), 0, 16, stream));
+    for (size_t k = 0; k < nf; ++k) {
+      if (specs[k].type != DType::Int64 && specs[k].type != DType::Float64) continue;
+      KernelTimer t("json_quoted_numbers_kernel", stream);
+      json_quoted_numbers_kernel<<<(unsigned)ceil_div(rows, 256), 256, 0, stream>>>(data, rows, specs[k].type == DType::Int64, (long long*)table[k].values,
+                                                                                   table[k].valid_bytes, (int32_t*)err.get());
+    }
+    ARK_CUDA(cudaMemcpyAsync(h.get(), err.get(), 16, cudaMemcpyDeviceToHost, stream));
+    ARK_CUDA(cudaStreamSynchronize(stream));
+    if (e[0] != JE_NONE) raise_json(e[0], e[1], "row");
+  }
   out_cols.clear();
   for (size_t k = 0; k < nf; ++k) {
     const InferredField& f = specs[k];

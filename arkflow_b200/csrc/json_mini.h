@@ -98,6 +98,20 @@ class JsonParser {
     } else err(std::string("unexpected character '") + c + "'");
     return v;
   }
+  // four hex digits at p_ (serde_json: anything else is an error)
+  unsigned hex4() {
+    if (p_ + 4 > s_.size()) err("bad \\u escape");
+    unsigned v = 0;
+    for (int k = 0; k < 4; ++k) {
+      const char h = s_[p_++];
+      const int d = h >= '0' && h <= '9' ? h - '0' : h >= 'a' && h <= 'f' ? h - 'a' + 10 : h >= 'A' && h <= 'F' ? h - 'A' + 10 : -1;
+      if (d < 0) err("bad \\u escape");
+      v = v * 16 + (unsigned)d;
+    }
+    return v;
+  }
+  // a JSON string → UTF-8.  Only JSON's nine escapes; a surrogate escape must be a high + low pair (combined into one
+  // code point, as the device decoder does); raw control characters are errors, as in serde_json.
   std::string string() {
     std::string out;
     ++p_;
@@ -105,21 +119,31 @@ class JsonParser {
       if (p_ >= s_.size()) err("unterminated string");
       char c = s_[p_++];
       if (c == '"') break;
+      if ((unsigned char)c < 0x20) err("control character in string");
       if (c == '\\') {
         if (p_ >= s_.size()) err("bad escape");
         char e = s_[p_++];
         switch (e) {
           case 'n': out += '\n'; break; case 't': out += '\t'; break; case 'r': out += '\r'; break;
           case 'b': out += '\b'; break; case 'f': out += '\f'; break;
+          case '"': case '\\': case '/': out += e; break;
           case 'u': {
-            if (p_ + 4 > s_.size()) err("bad \\u escape");
-            unsigned cp = (unsigned)strtoul(s_.substr(p_, 4).c_str(), nullptr, 16); p_ += 4;
+            unsigned cp = hex4();
+            if (cp >= 0xDC00 && cp <= 0xDFFF) err("lone low surrogate in \\u escape");
+            if (cp >= 0xD800 && cp <= 0xDBFF) {
+              if (p_ + 2 > s_.size() || s_[p_] != '\\' || s_[p_ + 1] != 'u') err("unpaired surrogate in \\u escape");
+              p_ += 2;
+              const unsigned lo = hex4();
+              if (lo < 0xDC00 || lo > 0xDFFF) err("unpaired surrogate in \\u escape");
+              cp = 0x10000 + ((cp - 0xD800) << 10) + (lo - 0xDC00);
+            }
             if (cp < 0x80) out += (char)cp;
             else if (cp < 0x800) { out += (char)(0xC0 | (cp >> 6)); out += (char)(0x80 | (cp & 0x3F)); }
-            else { out += (char)(0xE0 | (cp >> 12)); out += (char)(0x80 | ((cp >> 6) & 0x3F)); out += (char)(0x80 | (cp & 0x3F)); }
+            else if (cp < 0x10000) { out += (char)(0xE0 | (cp >> 12)); out += (char)(0x80 | ((cp >> 6) & 0x3F)); out += (char)(0x80 | (cp & 0x3F)); }
+            else { out += (char)(0xF0 | (cp >> 18)); out += (char)(0x80 | ((cp >> 12) & 0x3F)); out += (char)(0x80 | ((cp >> 6) & 0x3F)); out += (char)(0x80 | (cp & 0x3F)); }
             break;
           }
-          default: out += e;
+          default: err(std::string("bad escape '\\") + e + "'");
         }
       } else out += c;
     }

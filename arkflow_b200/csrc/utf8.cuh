@@ -1,11 +1,12 @@
 // utf8.cuh — well-formed UTF-8 per Unicode table 3-7 (no overlongs, no surrogates, ≤ U+10FFFF): the check
-// Rust's str::from_utf8 makes, used by CAST(Binary AS Utf8) and by the protobuf decoder's `string` fields.
+// Rust's str::from_utf8 makes, used by CAST(Binary AS Utf8), the protobuf decoder's `string` fields, the JSON
+// decoder's strings and schema inference, and the CSV input's Utf8 fields and header.
 #pragma once
 #include <cstdint>
 
 namespace ark {
 
-__device__ __forceinline__ bool utf8_valid(const uint8_t* p, long long len) {
+__host__ __device__ __forceinline__ bool utf8_valid(const uint8_t* p, long long len) {
   long long i = 0;
   while (i < len) {
     const uint8_t b0 = p[i];

@@ -116,6 +116,23 @@ def _to_f64(text: bytes) -> float:
     return float(text)
 
 
+def _check_no_surrogates(v):
+    stack = [v]
+    while stack:
+        x = stack.pop()
+        if isinstance(x, str):
+            try:
+                x.encode("utf-8")
+            except UnicodeEncodeError:
+                raise OracleError("Process", "Arrow JSON Reader Error: Json error: invalid string: unpaired surrogate escape")
+        elif isinstance(x, list):
+            stack.extend(x)
+        elif isinstance(x, tuple) and x[0] == "obj":
+            for k, e in x[1]:
+                stack.append(k)
+                stack.append(e)
+
+
 def json_to_arrow(rb: pa.RecordBatch, value_field: str = "__value__", fields_to_include: Optional[set] = None) -> pa.RecordBatch:
     if value_field not in rb.schema.names:
         raise OracleError("Process", "not found column")
@@ -131,6 +148,11 @@ def json_to_arrow(rb: pa.RecordBatch, value_field: str = "__value__", fields_to_
         values = list(_iter_values(data))
     except (ValueError, json.JSONDecodeError) as e:
         raise OracleError("Process", f"Arrow JSON Reader Error: Json error: {e}")
+    # Python's json decodes a lone or mispaired surrogate escape ("\ud800", "\udc00", "\ud800A") to a surrogate
+    # code point, which no UTF-8 string can hold; an arrow-rs StringArray is always valid UTF-8, so such a string is
+    # a Process error wherever it stands: a key, a value, an unknown field or inside a nested value.
+    for v in values:
+        _check_no_surrogates(v)
     if not values:
         return pa.RecordBatch.from_arrays([], schema=pa.schema([]))
     first = values[0]
