@@ -328,10 +328,18 @@ struct DenseGroups {  // result of the hash pass: dense arrays of G groups, part
 };
 
 bool launch_hash_agg_tile(const AggParams& P, unsigned long long capacity, unsigned int groups_hint, int64_t key_bytes, cudaStream_t stream);
-bool launch_hash_agg_stream(const AggParams& P, unsigned long long capacity, int64_t key_bytes, cudaStream_t stream);
-bool launch_hash_agg_radix(const AggParams& P, unsigned long long capacity, int32_t* skew_dev, std::vector<BufferPtr>* keep, cudaStream_t stream);
-void hash_agg_radix_note_skew();
+bool launch_hash_agg_stream(const AggParams& P, unsigned long long capacity, int64_t key_bytes, int forced, cudaStream_t stream);
 
+// ARK_AGG_KERNEL=staged|stream|general forces that table kernel, so that tests can run each one at small sizes; forcing
+// one also turns the tile kernel off.  Unset or any other value: the automatic choice.
+static int forced_agg_kernel() {
+  static const int k = [] {
+    const char* e = getenv("ARK_AGG_KERNEL");
+    const std::string v = e ? e : "";
+    return v == "staged" ? AGG_KERNEL_STAGED : v == "stream" ? AGG_KERNEL_STREAM : v == "general" ? AGG_KERNEL_GENERAL : AGG_KERNEL_AUTO;
+  }();
+  return k;
+}
 
 // dense, partition-ordered slot list of a built table (n_parts = 1: plain compaction)
 static void compact_groups(DenseGroups& dg, const ColView& kc, int key_kind, int n_parts, BufferPtr ctl, BufferPtr hctl, cudaStream_t stream);
@@ -343,14 +351,13 @@ static DenseGroups hash_pass(const Plan& plan, const AggExec& ex, Batch& in, int
   unsigned long long capacity = std::max<unsigned long long>(hints.capacity.load(), 1ull << 10);
   const unsigned long long cap_limit = 1ull << 31;
   DenseGroups dg;
-  BufferPtr ctl = device_alloc(512);  // [group_count u32 | overflow i32 | error i32 | skew i32 | part_counts u32[32] | part_cursor u32[32]]
+  BufferPtr ctl = device_alloc(512);  // [group_count u32 | overflow i32 | error i32 | pad | part_counts u32[32] @ 16 | part_cursor u32[32] @ 144 | long_seen i32 @ 280]
   BufferPtr hctl = pinned_alloc(512);
-  bool allow_radix = true;
   if (n_parts > 32) fail(ARK_ERR_UNSUPPORTED, "more than 32 partitions");
-  static const unsigned long long tile_max = [] { const char* e = getenv("ARK_AGG_TILE_MAX"); return e ? (unsigned long long)atoll(e) : 1024ull; }();  // 2048 slots (≈ 1000 groups): 1.65 ms in the tile kernel vs 1.34 ms in hash_agg_kernel
-  static const bool cache_enabled = [] { const char* e = getenv("ARK_AGG_TABLE_CACHE"); return !e || atoi(e) != 0; }();
+  const int forced = forced_agg_kernel();
+  const unsigned long long tile_max = forced ? 0 : 1024;  // 2048 slots (≈ 1000 groups): 1.65 ms in the tile kernel vs 1.34 ms in hash_agg_kernel
   // reuse needs self-contained keys (no row references) and a COUNT(*) accumulator that tells this batch's groups apart
-  const bool can_cache = cache_enabled && (ex.key_kind == KEY_INT64 || ex.key_kind == KEY_BYTES || ex.key_kind == KEY_BOOL) &&
+  const bool can_cache = (ex.key_kind == KEY_INT64 || ex.key_kind == KEY_BYTES || ex.key_kind == KEY_BOOL) &&
                          !ex.accs.empty() && (ex.accs[0].kind == ACC_COUNT_STAR || merge_mode);
   bool fresh_only = false;
   while (true) {
@@ -394,15 +401,12 @@ static DenseGroups hash_pass(const Plan& plan, const AggExec& ex, Batch& in, int
     P.long_seen = (int32_t*)((char*)ctl.get() + 280);
     P.max_groups = (unsigned int)std::min<unsigned long long>(capacity - capacity / 4, 0x7FFFFFFFull);  // retry above load 0.75
     ARK_CUDA(cudaMemsetAsync(ctl.get(), 0, 512, stream));
-    // large tables: partition rows by table region, build each region in shared memory (hash_agg_radix.cu)
-    std::vector<BufferPtr> radix_keep;
-    const bool radix = !reused && allow_radix && n > 0 && ex.key_kind != KEY_PAIR && launch_hash_agg_radix(P, capacity, (int32_t*)((char*)ctl.get() + 12), &radix_keep, stream);
     if (reused) {
       KernelTimer t("agg_reset_acc_kernel", stream);
       const int grid = (int)std::min<unsigned long long>((capacity * P.n_acc + 255) / 256, 148ull * 8);
       agg_reset_acc_kernel<<<grid, 256, 0, stream>>>(P.table, capacity, stride, P.n_acc, P.accs[0], P.accs[1], P.accs[2], P.accs[3], P.accs[4],
                                                      P.accs[5], P.accs[6], P.accs[7]);
-    } else if (!radix) {
+    } else {
       KernelTimer t("agg_init_kernel", stream);
       const int grid = (int)std::min<unsigned long long>((capacity + 255) / 256, 148ull * 8);
       agg_init_kernel<<<grid, 256, 0, stream>>>(P.table, capacity, stride, P.n_acc, P.accs[0], P.accs[1], P.accs[2], P.accs[3], P.accs[4],
@@ -425,9 +429,8 @@ static DenseGroups hash_pass(const Plan& plan, const AggExec& ex, Batch& in, int
     }
     // low cardinality (table ≤ 1024 slots): per-CTA hash table in shared memory (hash_agg_tile.cu) — hot keys would
     // serialise on L2 atomics here.  Everything larger: this file's row kernel.
-    if (radix) {
-    } else if (n > 0 && !reused && capacity <= tile_max && ex.key_kind != KEY_PAIR && launch_hash_agg_tile(P, capacity, hints.groups.load(), key_bytes, stream)) {
-    } else if (n > 0 && launch_hash_agg_stream(P, capacity, key_bytes, stream)) {
+    if (n > 0 && !reused && capacity <= tile_max && ex.key_kind != KEY_PAIR && launch_hash_agg_tile(P, capacity, hints.groups.load(), key_bytes, stream)) {
+    } else if (n > 0 && forced != AGG_KERNEL_GENERAL && launch_hash_agg_stream(P, capacity, key_bytes, forced, stream)) {
     } else {
       if (P.pred_kind == 0) launch_agg<0>(P, n, stream);
       else if (P.pred_kind == 1) launch_agg<1>(P, n, stream);
@@ -445,11 +448,6 @@ static DenseGroups hash_pass(const Plan& plan, const AggExec& ex, Batch& in, int
     const bool long_seen = *(int32_t*)((char*)hctl.get() + 280) != 0;
     if (reused && (overflow || groups > P.max_groups)) {  // the dictionary filled up with keys of past batches: start over at this size
       fresh_only = true;
-      continue;
-    }
-    if (*(int32_t*)((char*)hctl.get() + 12)) {  // skewed keys overflowed a bucket's record array: same capacity, row kernel
-      hash_agg_radix_note_skew();
-      allow_radix = false;
       continue;
     }
     if (overflow || groups > P.max_groups) {
@@ -858,8 +856,7 @@ bool run_group_by_merge(const Plan& plan, DistCtx& d, Batch& out, cudaStream_t s
   dg.n_acc = (int)ex.accs.size();
   BufferPtr ctl = device_alloc(512), hctl = pinned_alloc(512);
   bool poisoned = false, fresh_only = false;
-  static const bool cache_env = [] { const char* e = getenv("ARK_AGG_TABLE_CACHE"); return !e || atoi(e) != 0; }();
-  const bool cache_enabled = cache_env && mx.key_kind != KEY_NONE;  // a global aggregate's single group exists even with COUNT(*) = 0
+  const bool cache_enabled = mx.key_kind != KEY_NONE;  // a global aggregate's single group exists even with COUNT(*) = 0
   while (true) {
     // the owner meets the same keys step after step: keep the merge table's keys, reset its accumulators (AggHints::CachedTable)
     AggHints::CachedTable ct;

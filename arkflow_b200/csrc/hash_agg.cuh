@@ -58,6 +58,9 @@ __host__ __device__ inline bool acc_reads_values(int kind) { return kind != ACC_
 
 enum KeyKind : int32_t { KEY_NONE = 0, KEY_INT64 = 1, KEY_BYTES = 2, KEY_BOOL = 3, KEY_PAIR = 4 /* two key columns */ };
 
+// the table kernel ARK_AGG_KERNEL forces (hash_agg.cu); AGG_KERNEL_AUTO: chosen from the table size and the query
+enum AggKernel : int32_t { AGG_KERNEL_AUTO = 0, AGG_KERNEL_STREAM = 1, AGG_KERNEL_STAGED = 2, AGG_KERNEL_GENERAL = 3 };
+
 constexpr int AGG_MAX_ACC = 8;
 constexpr int AGG_MAX_PROGS = 2;
 

@@ -1,5 +1,4 @@
-// smem_table.cuh — open-addressing table of Key16 keys in shared memory (the partitioned GROUP BY's bucket regions
-// and the low-cardinality GROUP BY's per-CTA table).
+// smem_table.cuh — open-addressing table of Key16 keys in shared memory (the low-cardinality GROUP BY's per-CTA table).
 #pragma once
 #include "hash_agg.cuh"
 #include "hashkey.cuh"

@@ -17,17 +17,6 @@ run "filter pipe nolookback"       ARK_FP_IMPL=0 ARK_FP_DEBUG=1 timeout 300 pyth
 run "filter r1 kernel"             ARK_FP_IMPL=1 timeout 300 python scripts/prof_query.py "$FQ" 16777216 1000000 20 0 6
 run "filter fixed-only pipe"       ARK_FP_IMPL=0 timeout 300 python scripts/prof_query.py "SELECT timestamp, value FROM flow WHERE value >= 10" 16777216 1000000 20 0 6
 run "filter fixed-only r1"         ARK_FP_IMPL=1 timeout 300 python scripts/prof_query.py "SELECT timestamp, value FROM flow WHERE value >= 10" 16777216 1000000 20 0 6
-run "groupby stream R2"            ARK_AGG_STREAM=1 timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
-run "groupby stream R1"            ARK_AGG_STREAM=1 ARK_AGG_STREAM_R=1 timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
-run "groupby stream R4"            ARK_AGG_STREAM=1 ARK_AGG_STREAM_R=4 timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
-run "groupby generic kernel"       ARK_AGG_STREAM=0 timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
-run "groupby stream R2 K=1e5"      ARK_AGG_STREAM=1 timeout 300 python scripts/prof_query.py "$GQ" 16777216 100000 12 0 3
-run "groupby stream R1 K=1e5"      ARK_AGG_STREAM=1 ARK_AGG_STREAM_R=1 timeout 300 python scripts/prof_query.py "$GQ" 16777216 100000 12 0 3
-run "groupby generic K=1e5"        ARK_AGG_STREAM=0 timeout 300 python scripts/prof_query.py "$GQ" 16777216 100000 12 0 3
-run "groupby stream R2 K=4e6"      ARK_AGG_STREAM=1 timeout 300 python scripts/prof_query.py "$GQ" 16777216 4000000 12 0 3
-run "groupby stream R1 K=4e6"      ARK_AGG_STREAM=1 ARK_AGG_STREAM_R=1 timeout 300 python scripts/prof_query.py "$GQ" 16777216 4000000 12 0 3
-run "groupby generic K=4e6"        ARK_AGG_STREAM=0 timeout 300 python scripts/prof_query.py "$GQ" 16777216 4000000 12 0 3
-run "groupby int key K~1e6"        ARK_AGG_STREAM=1 timeout 300 python scripts/prof_query.py "SELECT timestamp, SUM(value), COUNT(*) FROM flow GROUP BY timestamp" 2000000 1000000 12 0 3
 cat $OUT/ab.log
 timeout 600 ncu --set full --clock-control none --import-source on -k regex:filter_project_pipe -s 6 -c 2 -o $OUT/fp_pipe python scripts/prof_query.py "$FQ" 16777216 1000000 4 0 3 > $OUT/ncu_fp.log 2>&1
 timeout 600 ncu --set full --clock-control none --import-source on -k regex:hash_agg_stream -s 6 -c 2 -o $OUT/agg_stream python scripts/prof_query.py "$GQ" 16777216 1000000 4 0 3 > $OUT/ncu_agg.log 2>&1

@@ -16,17 +16,7 @@ run "filter pipe minb5"            ARK_FP_IMPL=0 ARK_FP_MINB=5 timeout 300 pytho
 run "filter r1 kernel"             ARK_FP_IMPL=1 timeout 300 python scripts/prof_query.py "$FQ" 16777216 1000000 20 0 6
 run "filter fixed-only tile"       ARK_FP_IMPL=2 timeout 300 python scripts/prof_query.py "SELECT timestamp, value FROM flow WHERE value >= 10" 16777216 1000000 20 0 6
 run "filter fixed-only r1"         ARK_FP_IMPL=1 timeout 300 python scripts/prof_query.py "SELECT timestamp, value FROM flow WHERE value >= 10" 16777216 1000000 20 0 6
-run "groupby stream R1"            ARK_AGG_STREAM_R=1 timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
-run "groupby stream R2"            ARK_AGG_STREAM_R=2 timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
-run "groupby R1 noRED"             ARK_AGG_STREAM_R=1 ARK_AGG_DEBUG=1 timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
-run "groupby R1 noprobe"           ARK_AGG_STREAM_R=1 ARK_AGG_DEBUG=2 timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
-run "groupby R1 noprobe noRED"     ARK_AGG_STREAM_R=1 ARK_AGG_DEBUG=3 timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
-run "groupby R1 stream only"       ARK_AGG_STREAM_R=1 ARK_AGG_DEBUG=7 timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
-run "groupby R1 notable+RED"       ARK_AGG_STREAM_R=1 ARK_AGG_DEBUG=6 timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
-run "groupby R2 stream only"       ARK_AGG_STREAM_R=2 ARK_AGG_DEBUG=7 timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
-run "groupby generic kernel"       ARK_AGG_STREAM=0 timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
 cat $OUT/ab.log
 timeout 600 ncu --set full --clock-control none --import-source on -k regex:filter_project_tile -s 6 -c 2 -o $OUT/fp_tile python scripts/prof_query.py "$FQ" 16777216 1000000 4 0 3 > $OUT/ncu_fp.log 2>&1
-ARK_AGG_STREAM_R=1 timeout 600 ncu --set full --clock-control none --import-source on -k regex:hash_agg_stream -s 6 -c 2 -o $OUT/agg_stream_r1 python scripts/prof_query.py "$GQ" 16777216 1000000 4 0 3 > $OUT/ncu_agg.log 2>&1
 timeout 900 python bench.py --steps 20 --warmup 5 > $OUT/bench.json 2> $OUT/bench.err; echo "bench rc=$?"; tail -c 3000 $OUT/bench.json; tail -5 $OUT/bench.err
 ls -la $OUT

@@ -22,13 +22,6 @@ run "filter r1 kernel"                  ARK_FP_IMPL=1 timeout 300 python scripts
 run "filter fixed-only dt256"           timeout 300 python scripts/prof_query.py "SELECT timestamp, value FROM flow WHERE value >= 10" 16777216 1000000 20 0 6
 run "filter fixed-only dt512 lbw8"      ARK_FP_THREADS=512 ARK_FP_MINB=2 ARK_FP_LB_WINDOWS=8 timeout 300 python scripts/prof_query.py "SELECT timestamp, value FROM flow WHERE value >= 10" 16777216 1000000 20 0 6
 run "groupby staged R1 cached"          timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
-run "groupby staged R2 cached"          ARK_AGG_STREAM_R=2 timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
-run "groupby staged R1 nocache"         ARK_AGG_TABLE_CACHE=0 timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
-run "groupby v1 R1 cached"              ARK_AGG_STREAM_V=1 timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
-run "groupby staged stream-only"        ARK_AGG_DEBUG=7 ARK_AGG_TABLE_CACHE=0 timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
-run "groupby staged R2 stream-only"     ARK_AGG_STREAM_R=2 ARK_AGG_DEBUG=7 ARK_AGG_TABLE_CACHE=0 timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
-run "groupby staged noRED cached"       ARK_AGG_DEBUG=1 timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
-run "groupby generic cached"            ARK_AGG_STREAM=0 timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
 run "groupby staged K=1e5 cached"       timeout 300 python scripts/prof_query.py "$GQ" 16777216 100000 12 0 3
 run "groupby staged K=4e6 cached"       timeout 300 python scripts/prof_query.py "$GQ" 16777216 4000000 12 0 3
 cat $OUT/ab.log

@@ -6,9 +6,6 @@ mkdir -p $OUT
 GQ="SELECT sensor, SUM(value), COUNT(*) FROM flow GROUP BY sensor"
 run() { echo "== $1" >> $OUT/ab.log; shift; env "$@" 2>&1 | grep -v "^agg_\(emit\|gather\|finalize\)" >> $OUT/ab.log; }
 run "groupby staged K=1e6 cached"   timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
-run "groupby staged K=1e6 nocache"  ARK_AGG_TABLE_CACHE=0 timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
-run "groupby staged K=1e6 3 CTAs"   ARK_AGG_STREAM_CTAS=3 timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
-run "groupby staged K=1e6 noRED"    ARK_AGG_DEBUG=1 timeout 300 python scripts/prof_query.py "$GQ" 16777216 1000000 12 0 3
 run "groupby staged K=1e5"          timeout 300 python scripts/prof_query.py "$GQ" 16777216 100000 12 0 3
 run "groupby staged K=4e6"          timeout 300 python scripts/prof_query.py "$GQ" 16777216 4000000 12 0 3
 run "groupby staged K=1e4"          timeout 300 python scripts/prof_query.py "$GQ" 16777216 10000 12 0 3

@@ -40,7 +40,7 @@ for i in range(reps):
     proc.process_device(bs[i % nres]).close()
 torch.cuda.synchronize()
 print(f"call wall avg {(time.perf_counter() - t0) / reps * 1e3:.3f} ms")
-for name in (b"hash_agg_staged_kernel", b"hash_agg_stream_kernel", b"hash_agg_kernel", b"hash_agg_tile_kernel", b"filter_project_tma_kernel", b"filter_project_kernel", b"agg_radix_partition_kernel", b"agg_radix_bucket_kernel", b"agg_init_kernel", b"agg_compact_kernel", b"agg_emit_keys_kernel", b"agg_gather_acc_kernel", b"agg_finalize_kernel"):
+for name in (b"hash_agg_staged_kernel", b"hash_agg_stream_kernel", b"hash_agg_kernel", b"hash_agg_tile_kernel", b"filter_project_tma_kernel", b"filter_project_kernel", b"agg_init_kernel", b"agg_compact_kernel", b"agg_emit_keys_kernel", b"agg_gather_acc_kernel", b"agg_finalize_kernel"):
     ms, n = C.c_double(), C.c_int64()
     lib.ark_kernel_timing_get(name, C.byref(ms), C.byref(n))
     if n.value:

@@ -2,13 +2,12 @@
 
 Several implementations accumulate into the same table (DESIGN.md §4.2), each with its own accumulate, merge and
 identity logic: the per-CTA shared-memory table (hash_agg_tile_kernel; ≤ 64 slots reduce in the warp first), the
-TMA-staged kernel (hash_agg_staged_kernel, R = 1 / 2), the register-prefetch kernel (hash_agg_stream_kernel,
-R = 1 / 2 / 4), the general row kernel (hash_agg_kernel), the partitioned path (agg_radix_*) and a cached key
-dictionary whose accumulators agg_reset_acc_kernel resets.  The knobs that pick a kernel are read once per process, so
-each path runs in a child process: this process builds the inputs and the oracle's answers, the child runs the library
-and writes its results as Arrow IPC together with the kernels each call launched.  Every case asserts that the
-intended kernel ran, or that the path declines the case by design (VM predicate, two keys, Boolean key, more than six
-accumulators for the tile kernel): a silent fallback fails.
+TMA-staged kernel (hash_agg_staged_kernel), the register-prefetch kernel (hash_agg_stream_kernel), the general row
+kernel (hash_agg_kernel) and a cached key dictionary whose accumulators agg_reset_acc_kernel resets.  ARK_AGG_KERNEL,
+which forces a kernel, is read once per process, so each path runs in a child process: this process builds the inputs
+and the oracle's answers, the child runs the library and writes its results as Arrow IPC together with the kernels
+each call launched.  Every case asserts that the intended kernel ran, or that the path declines the case by design (VM
+predicate, two keys, Boolean key, more than six accumulators for the tile kernel): a silent fallback fails.
 
 Comparison: keys, integers and counts exactly; Float64 MIN / MAX bitwise (totalOrder separates -0.0 from +0.0 and NaN
 payloads); Float64 SUM / AVG by tests/agg_util.py (NaN ↔ NaN, ±inf exact, else the §7 bound).
@@ -29,7 +28,7 @@ pytestmark = pytest.mark.gpu
 
 I64_MIN, I64_MAX = -2 ** 63, 2 ** 63 - 1
 TABLE_KERNELS = ("hash_agg_tile_kernel", "hash_agg_staged_kernel", "hash_agg_stream_kernel", "hash_agg_kernel")
-KERNELS = TABLE_KERNELS + ("agg_radix_bucket_kernel", "agg_reset_acc_kernel")
+KERNELS = TABLE_KERNELS + ("agg_reset_acc_kernel",)
 # quiet and signalling NaNs of both signs; 0x7FFF… and 0xFFFF… have the totalOrder keys INT64_MAX / INT64_MIN, the
 # identities of the MIN / MAX accumulators
 NAN_BITS = np.array([0x7FF8000000000000, 0xFFF8000000000000, 0x7FF0000000000001, 0x7FFFFFFFFFFFFFFF, 0xFFFFFFFFFFFFFFFF,
@@ -129,8 +128,8 @@ Q_FLT = "SELECT {K}, SUM(f), AVG(f), MIN(f), MAX(f), COUNT(f) FROM flow{W} GROUP
 Q_CNT = "SELECT {K}, COUNT(*), COUNT(i), COUNT(f), COUNT(s), COUNT(b), COUNT(t) FROM flow{W} GROUP BY {K}"
 Q_WIDE = "SELECT {K}, SUM(j), AVG(j), MIN(i), MAX(f), COUNT(s), COUNT(*) FROM flow{W} GROUP BY {K}"  # 8 accumulators
 Q_ARGS3 = "SELECT {K}, SUM(j), MAX(m), MIN(h), AVG(h) FROM flow{W} GROUP BY {K}"  # 3rd argument is loaded in place
-Q_RADIX = "SELECT {K}, COUNT(*), SUM(j), MIN(j), MAX(m), AVG(j) FROM flow{W} GROUP BY {K}"  # non-null, ≤ 2 arguments
-Q_RADIX_F = "SELECT {K}, SUM(h), MAX(h), MIN(h), COUNT(*) FROM flow{W} GROUP BY {K}"
+Q_NONNULL = "SELECT {K}, COUNT(*), SUM(j), MIN(j), MAX(m), AVG(j) FROM flow{W} GROUP BY {K}"  # non-null, ≤ 2 arguments
+Q_NONNULL_F = "SELECT {K}, SUM(h), MAX(h), MIN(h), COUNT(*) FROM flow{W} GROUP BY {K}"
 Q_AUX = "SELECT {K}, COUNT(f), SUM(af), COUNT(i), SUM(ai), COUNT(j), SUM(aj), COUNT(h), SUM(ah) FROM flow{W} GROUP BY {K}"
 W_INT, W_FLT, W_FLT2, W_VM = " WHERE p > 0", " WHERE q < 0.0", " WHERE q >= 1.5", " WHERE p > 0 AND q < 0.5"
 FLOAT_SUMS = {"sum(flow.f)": "f", "avg(flow.f)": "f", "avg(flow.i)": "i", "avg(flow.j)": "j", "avg(flow.h)": "h",
@@ -164,13 +163,9 @@ PRED = [(Q_INT, W_INT), (Q_FLT, W_FLT), (Q_ARGS3, W_FLT2), (Q_CNT, W_VM)]
 
 PATHS = {  # name → (environment, kernel it selects)
     "tile": ({}, "hash_agg_tile_kernel"),
-    "staged_r1": ({"ARK_AGG_STREAM_V": "2", "ARK_AGG_STREAM_R": "1", "ARK_AGG_TILE_MAX": "0"}, "hash_agg_staged_kernel"),
-    "staged_r2": ({"ARK_AGG_STREAM_V": "2", "ARK_AGG_STREAM_R": "2", "ARK_AGG_TILE_MAX": "0"}, "hash_agg_staged_kernel"),
-    "stream_r1": ({"ARK_AGG_STREAM_V": "1", "ARK_AGG_STREAM_R": "1", "ARK_AGG_TILE_MAX": "0"}, "hash_agg_stream_kernel"),
-    "stream_r2": ({"ARK_AGG_STREAM_V": "1", "ARK_AGG_STREAM_R": "2", "ARK_AGG_TILE_MAX": "0"}, "hash_agg_stream_kernel"),
-    "stream_r4": ({"ARK_AGG_STREAM_V": "1", "ARK_AGG_STREAM_R": "4", "ARK_AGG_TILE_MAX": "0"}, "hash_agg_stream_kernel"),
-    "general": ({"ARK_AGG_STREAM": "0", "ARK_AGG_TILE_MAX": "0"}, "hash_agg_kernel"),
-    "radix": ({"ARK_AGG_RADIX": "2"}, "agg_radix_bucket_kernel"),
+    "staged": ({"ARK_AGG_KERNEL": "staged"}, "hash_agg_staged_kernel"),
+    "stream": ({"ARK_AGG_KERNEL": "stream"}, "hash_agg_stream_kernel"),
+    "general": ({"ARK_AGG_KERNEL": "general"}, "hash_agg_kernel"),
 }
 
 
@@ -186,11 +181,6 @@ def _cases(path):
         query = q.format(K=_keys_of(table), W=w)
         out.append((f"{path}-{len(out)}", table, query, calls, off, device))
 
-    if path == "radix":
-        for t in ("u_hi", "i_hi", "u_big"):
-            add(t, Q_RADIX)
-            add(t, Q_RADIX_F, W_FLT)
-        return out
     # the tile kernel: ≤ 16 groups from the second call of a processor on (≤ 64 slots), a few hundred groups
     calls = 2 if path == "tile" else 1
     tables = LOW + MID + ([] if path == "tile" else HIGH)
@@ -203,7 +193,10 @@ def _cases(path):
     if path != "tile":
         for q in (Q_INT, Q_ARGS3, Q_CNT):
             add("u_big", q)
-    if path in ("tile", "staged_r1", "stream_r1"):  # device slices (and host slices) of the default, staged and prefetch paths
+        for t in HIGH + ["u_big"]:  # every argument non-null: the staged kernel stages both
+            add(t, Q_NONNULL)
+            add(t, Q_NONNULL_F, W_FLT)
+    if path in ("tile", "staged", "stream"):  # device slices (and host slices) of the default, staged and prefetch paths
         for off in (1, 3, 7, 1237):
             for t in ("sl_lo", "sl_hi", "sl_i"):
                 for device in (True, False):
@@ -213,10 +206,8 @@ def _cases(path):
 
 
 def _expected(path, table, query, call):
-    """(kernel that call number `call` of a case must have run, table kernels allowed to run; None: any)."""
+    """(kernel that call number `call` of a case must have run, table kernels allowed to run)."""
     env, kernel = PATHS[path]
-    if path == "radix":
-        return kernel, None
     key = TABLES[table].get("key", "utf8")
     if " AND " in query or key == "pair":  # VM predicate, two keys: only the general kernel takes them
         return "hash_agg_kernel", {"hash_agg_kernel"}
@@ -373,8 +364,7 @@ def _run_path(path, tmp, cases, check_kernels=True):
                 need, allowed = _expected(path, t, q, k)
                 counts = run["counts"]
                 assert counts[need] >= 1, (what, need, counts)
-                if allowed is not None:
-                    assert all(counts[x] == 0 for x in TABLE_KERNELS if x not in allowed), (what, allowed, counts)
+                assert all(counts[x] == 0 for x in TABLE_KERNELS if x not in allowed), (what, allowed, counts)
     return report
 
 

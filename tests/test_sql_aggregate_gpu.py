@@ -233,14 +233,7 @@ def test_aggregate_planning_errors(gpu):
         run(rb, "SELECT SUM(sensor) FROM flow")
 
 
-# ---- partitioned (radix) path: csrc/hash_agg_radix.cu ------------------------------------------------
-def _launches(lib, name):
-    import ctypes as C
-    ms, n = C.c_double(), C.c_int64()
-    lib.ark_kernel_timing_get(name.encode(), C.byref(ms), C.byref(n))
-    return n.value
-
-
+# ---- many groups: string, Int64, long and NULL keys, float values, one hot key --------------------------
 def check_agg_sorted(rb, query, key, float_cols=()):
     """check_agg for many groups: both results sorted by the key column, columns compared as arrays."""
     want = sql_process(rb, query)
@@ -261,27 +254,16 @@ def check_agg_sorted(rb, query, key, float_cols=()):
     return want
 
 
-@pytest.fixture
-def radix_mode(gpu, monkeypatch):
-    monkeypatch.setenv("ARK_AGG_RADIX", "2")  # take the partitioned path already from 2^16 rows / slots
-    gpu.ark_kernel_timing_reset()
-    gpu.ark_kernel_timing_enable(1)
-    yield gpu
-    gpu.ark_kernel_timing_enable(0)
-
-
-def test_radix_path_string_keys(radix_mode):
+def test_many_groups_string_keys(gpu):
     rb = synth_batch(400_000, key_space=150_000, seed=21)
     q = "SELECT sensor, SUM(value), COUNT(*) FROM flow GROUP BY sensor"
     check_agg_sorted(rb, q, "sensor")  # first call may still be growing the capacity hint
-    radix_mode.ark_kernel_timing_reset()
     check_agg_sorted(rb, q, "sensor")
-    assert _launches(radix_mode, "agg_radix_bucket_kernel") >= 2 and _launches(radix_mode, "hash_agg_kernel") == 0
     check_agg_sorted(rb, "SELECT sensor, SUM(value), COUNT(*), MIN(value), MAX(value), AVG(value) FROM flow WHERE value >= 4 GROUP BY sensor",
                      "sensor", float_cols=["avg(flow.value)"])
 
 
-def test_radix_path_float_values_and_int_keys(radix_mode):
+def test_many_groups_float_values_and_int_keys(gpu):
     rb = synth_batch(300_000, value_kind=1, key_space=120_000, seed=22)
     check_agg_sorted(rb, "SELECT sensor, SUM(value), AVG(value), COUNT(*) FROM flow GROUP BY sensor", "sensor",
                      float_cols=["sum(flow.value)", "avg(flow.value)"])
@@ -289,10 +271,9 @@ def test_radix_path_float_values_and_int_keys(radix_mode):
     n = 300_000
     rb2 = pa.record_batch({"id": pa.array(rng.integers(-2**40, 2**40, n) // 2**23, pa.int64()), "v": pa.array(rng.integers(-2**62, 2**62, n), pa.int64())})
     check_agg_sorted(rb2, "SELECT id, SUM(v), COUNT(*), MIN(v), MAX(v) FROM flow GROUP BY id", "id")
-    assert _launches(radix_mode, "agg_radix_bucket_kernel") >= 2
 
 
-def test_radix_path_long_keys_and_null_keys(radix_mode):
+def test_many_groups_long_keys_and_null_keys(gpu):
     rng = np.random.default_rng(24)
     n = 200_000
     ids = rng.integers(0, 90_000, n)
@@ -300,11 +281,10 @@ def test_radix_path_long_keys_and_null_keys(radix_mode):
     rb = pa.record_batch({"sensor": pa.array(keys, pa.utf8()), "value": pa.array(rng.integers(0, 1000, n), pa.int64())})
     want = check_agg_sorted(rb, "SELECT sensor, SUM(value), COUNT(*) FROM flow GROUP BY sensor", "sensor")
     assert want.column("sensor").null_count == 1
-    assert _launches(radix_mode, "agg_radix_bucket_kernel") >= 1
 
 
-def test_radix_path_skewed_keys_fall_back(radix_mode):
-    # half of the rows carry one key: that bucket's record array overflows, the batch is redone by hash_agg_kernel
+def test_many_groups_one_hot_key(gpu):
+    # half of the rows carry one key: its slot takes every other row's atomics
     rb = synth_batch(400_000, key_space=150_000, seed=25)
     hot = pa.array(["hot_sensor_0"] * 400_000)
     idx = np.arange(400_000)
@@ -312,9 +292,7 @@ def test_radix_path_skewed_keys_fall_back(radix_mode):
     rb = pa.record_batch({"timestamp": rb.column("timestamp"), "value": rb.column("value"), "sensor": sensor})
     q = "SELECT sensor, SUM(value), COUNT(*) FROM flow GROUP BY sensor"
     check_agg_sorted(rb, q, "sensor")
-    radix_mode.ark_kernel_timing_reset()
     check_agg_sorted(rb, q, "sensor")
-    assert _launches(radix_mode, "agg_radix_partition_kernel") >= 1 and _launches(radix_mode, "hash_agg_kernel") >= 1
 
 
 def test_protobuf_example_query_cast_of_aggregate_and_order_by(gpu):
