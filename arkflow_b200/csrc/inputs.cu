@@ -12,12 +12,22 @@
 //               lines are decoded by the json_to_arrow kernels (csrc/json.cu), CSV rows by csv_parse_kernel; the
 //               optional query runs through the sql processor.  Parquet / Avro / Arrow IPC and remote object stores
 //               are not read here (ARK_ERR_UNSUPPORTED; SURVEY.md §8(f) rank 4 names CSV / JSON first).
-//               Deviations from DataFusion's readers: the JSON schema is inferred from the first record (as the
-//               json_to_arrow processor does; DataFusion samples 1000), CSV types from the first 1000 rows with the
+//               The NDJSON schema is merged over the first 1000 records and fixed for the file, as DataFusion does.
+//               Deviations from DataFusion's readers: CSV types come from the first 1000 records with the
 //               types Int64 / Float64 / Boolean / Utf8 (dates stay strings), quoted CSV fields may not contain line
-//               breaks.  A CSV column is Int64 when its sample values are decimal integers within the i64 range, and
+//               breaks (oracle/csv_oracle.py lists the smaller ones).  A CSV column is Int64 when its sample values are decimal integers within the i64 range, and
 //               Float64 when they are decimals or nan / inf / infinity (any case, optional sign; Arrow's reader
 //               accepts these spellings too); Float64 values are correctly rounded.
+//               Lines: `\n` and `\r\n` both end a line, and the last line needs no terminator.  An empty line (nothing
+//               but `\r` before its `\n`) is not a record in either format, as in csv-core and arrow-json: it is left
+//               out of the line index, so it never counts toward `batch_size` and the CSV header is the first line
+//               that is not empty.  Every batch but the last therefore holds exactly `batch_size` lines; an NDJSON line
+//               of spaces only is a line that the decoder drops, so such a batch comes out shorter.
+//               CSV errors: a batch reports the error of its FIRST failing line in file order, and the line number in
+//               the message counts physical lines from 1, empty ones included.  Within one line the order is: wrong
+//               number of fields (bytes after a closing quote count as such), then a value that does not parse as its
+//               column's type (invalid UTF-8 in a numeric or Boolean field is this error), then invalid UTF-8 in a
+//               Utf8 field.  tests/test_inputs_edges_gpu.py checks all of this against oracle/csv_oracle.py.
 #include <sys/stat.h>
 
 #include <chrono>
@@ -28,6 +38,9 @@
 
 #include <cub/device/device_scan.cuh>
 #include <cub/device/device_select.cuh>
+
+#include <thrust/count.h>
+#include <thrust/execution_policy.h>
 
 #include "decimal.cuh"
 #include "engine.h"
@@ -80,17 +93,15 @@ std::chrono::nanoseconds parse_duration_in(const std::string& s) {
   return std::chrono::nanoseconds((long long)total);
 }
 
-// out[i*len .. (i+1)*len) = payload, offsets[i] = i*len; 16 bytes per thread
-__global__ void replicate_kernel(const uint8_t* payload, int len, long long n, uint8_t* out, int32_t* offsets) {
-  extern __shared__ uint8_t s_pay[];
-  for (int i = threadIdx.x; i < len; i += blockDim.x) s_pay[i] = payload[i];
-  __syncthreads();
+// out[i*len .. (i+1)*len) = payload, offsets[i] = i*len; 16 bytes per thread.  The payload is read through the
+// read-only cache: it has any length a Binary array admits, so it is not staged in shared memory.
+__global__ void replicate_kernel(const uint8_t* __restrict__ payload, int len, long long n, uint8_t* out, int32_t* offsets) {
   const long long total = n * len;
   for (long long p = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * 16; p < total; p += (long long)gridDim.x * blockDim.x * 16) {
     uint8_t v[16];
     int k = (int)(p % len);
 #pragma unroll
-    for (int b = 0; b < 16; ++b) { v[b] = s_pay[k]; if (++k == len) k = 0; }
+    for (int b = 0; b < 16; ++b) { v[b] = __ldg(payload + k); if (++k == len) k = 0; }
     if (p + 16 <= total) *reinterpret_cast<uint4*>(out + p) = *reinterpret_cast<const uint4*>(v);
     else for (int b = 0; p + b < total; ++b) out[p + b] = v[b];
   }
@@ -98,10 +109,18 @@ __global__ void replicate_kernel(const uint8_t* payload, int len, long long n, u
 }
 
 // ---- line index --------------------------------------------------------------------------------------------------
-// flags[i] = 1 when byte i starts a line (i == 0 or byte i-1 is '\n') and the line is not blank-to-end
+// flags[i] = 1 when byte i starts a line (i == 0 or byte i-1 is '\n') that is not empty: it has a byte other than
+// '\r' before its '\n' or the end of the file
 __global__ void line_start_flags_kernel(const uint8_t* data, long long n, uint8_t* flags) {
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
-    flags[i] = (i == 0 || data[i - 1] == '\n') ? 1 : 0;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    uint8_t f = 0;
+    if (i == 0 || data[i - 1] == '\n') {
+      long long j = i;
+      while (j < n && data[j] == '\r') ++j;
+      f = j < n && data[j] != '\n';
+    }
+    flags[i] = f;
+  }
 }
 
 // ---- CSV ---------------------------------------------------------------------------------------------------------
@@ -120,7 +139,8 @@ struct CsvParams {
   int32_t* str_len[CSV_MAX_COLS];    // Utf8: decoded length per row (n_rows + 1 entries; scanned into offsets)
   long long* str_src[CSV_MAX_COLS];  // Utf8: absolute position of the field body
   int32_t* str_raw[CSV_MAX_COLS];    // Utf8: raw length; negative ⇒ quoted field with "" escapes
-  int32_t* error;                    // [0] = 1 bad number / 2 wrong field count / 3 invalid UTF-8 in a Utf8 field, [1] = row
+  unsigned long long* error;         // min over the failing rows of row << 2 | code (all ones: none); code 1 = bad value,
+                                     // 2 = wrong field count, 3 = invalid UTF-8 in a Utf8 field
 };
 
 // The host's type inference (csv_infer_type) calls the same two grammar tests as the kernel, so a column inferred
@@ -165,12 +185,13 @@ __device__ inline bool csv_parse_f64(const uint8_t* p, int len, double* out) {
 }
 
 // One thread per row: split at the delimiter (quoted fields may hold delimiters and "" escapes), convert per type.
+// A failing row folds row << 2 | code into P.error with one atomicMin, so the batch reports its first failing row.
 __global__ void csv_parse_kernel(const __grid_constant__ CsvParams P) {
   for (long long row = (long long)blockIdx.x * blockDim.x + threadIdx.x; row < P.n_rows; row += (long long)gridDim.x * blockDim.x) {
     long long pos = P.line_off[row], end = P.line_off[row + 1];
     while (end > pos && (P.data[end - 1] == '\n' || P.data[end - 1] == '\r')) --end;
     int col = 0;
-    bool bad = false, bad_utf8 = false;
+    bool bad = false, bad_utf8 = false, few = false;
     while (col < P.n_cols) {
       long long f0 = pos, f1;
       bool escaped = false;
@@ -214,13 +235,12 @@ __global__ void csv_parse_kernel(const __grid_constant__ CsvParams P) {
           break;
         }
       }
-      ++col;
+      if (++col == P.n_cols) break;  // what is left of the line, a trailing delimiter too, is one field too many
       if (pos < end && P.data[pos] == (uint8_t)P.delim) ++pos;
-      else if (col < P.n_cols) { bad = true; for (; col < P.n_cols; ++col) { P.valid[col][row] = 0; if (P.types[col] == CSV_STR) { P.str_len[col][row] = 0; P.str_src[col][row] = 0; P.str_raw[col][row] = 0; } } if (atomicCAS(P.error, 0, 2) == 0) P.error[1] = (int32_t)row; break; }
+      else { few = true; for (; col < P.n_cols; ++col) { P.valid[col][row] = 0; if (P.types[col] == CSV_STR) { P.str_len[col][row] = 0; P.str_src[col][row] = 0; P.str_raw[col][row] = 0; } } }
     }
-    if (!bad && pos < end) { bad = true; if (atomicCAS(P.error, 0, 2) == 0) P.error[1] = (int32_t)row; }  // more fields than the header
-    else if (bad && atomicCAS(P.error, 0, 1) == 0) P.error[1] = (int32_t)row;
-    else if (bad_utf8 && atomicCAS(P.error, 0, 3) == 0) P.error[1] = (int32_t)row;
+    const int code = (few || pos < end) ? 2 : bad ? 1 : bad_utf8 ? 3 : 0;
+    if (code) atomicMin(P.error, ((unsigned long long)row << 2) | (unsigned long long)code);
   }
 }
 
@@ -253,8 +273,7 @@ struct ark_input {
   bool connected = false, closed = false;
   BufferPtr file_dev;       // the file's bytes in HBM
   int64_t file_bytes = 0;
-  BufferPtr line_off;       // int64 starts of the non-header lines (+ file end) on the device
-  std::vector<int64_t> line_off_host_tail;  // unused
+  BufferPtr line_off;       // int64 starts of the lines that are not empty (+ file end) on the device
   int64_t n_lines = 0, next_line = 0, rows_per_batch = 1 << 22;
   std::unique_ptr<Processor> decoder;
   std::unique_ptr<SqlProcessor> sql;
@@ -278,7 +297,7 @@ Batch generate_batch(ark_input* in, cudaStream_t stream) {
   if (len) ARK_CUDA(cudaMemcpyAsync(pay.get(), in->context.data(), (size_t)len, cudaMemcpyHostToDevice, stream));
   {
     KernelTimer t("replicate_kernel", stream);
-    replicate_kernel<<<grid_of(std::max<long long>((long long)len * n / 16, n + 1)), 256, (size_t)std::max(len, 1), stream>>>(
+    replicate_kernel<<<grid_of(std::max<long long>((long long)len * n / 16, n + 1)), 256, 0, stream>>>(
         (const uint8_t*)pay.get(), std::max(len, 0), n, (uint8_t*)data.get(), (int32_t*)off.get());
   }
   ARK_CUDA(cudaGetLastError());
@@ -376,6 +395,13 @@ Batch lines_batch(ark_input* in, int64_t l0, int64_t n, int64_t byte0, int64_t b
   return b;
 }
 
+// the 1-based physical line that holds byte `off` of the file: the line terminators before it, empty lines included
+long long physical_line(ark_input* in, long long off, cudaStream_t stream) {
+  const uint8_t* file = (const uint8_t*)in->file_dev.get();
+  note_launch("thrust::count");
+  return 1 + (long long)thrust::count(thrust::cuda::par.on(stream), file, file + off, (uint8_t)'\n');
+}
+
 std::vector<std::string> split_csv_line(const std::string& line, char delim) {
   std::vector<std::string> out;
   std::string cur;
@@ -415,8 +441,8 @@ int csv_infer_type(const std::string& f, int cur) {  // -1 = no evidence yet (on
 
 void csv_prepare(ark_input* in, cudaStream_t stream) {
   if (in->n_lines == 0) return;
-  // header + up to 1000 rows on the host
-  const int64_t sample_lines = std::min<int64_t>(in->n_lines, 1001);
+  // the header, when there is one, + up to 1000 rows on the host
+  const int64_t sample_lines = std::min<int64_t>(in->n_lines, (in->has_header ? 1 : 0) + 1000);
   std::vector<long long> starts((size_t)sample_lines + 1);
   ARK_CUDA(cudaMemcpyAsync(starts.data(), in->line_off.get(), (size_t)(sample_lines + 1) * 8, cudaMemcpyDeviceToHost, stream));
   ARK_CUDA(cudaStreamSynchronize(stream));
@@ -432,15 +458,13 @@ void csv_prepare(ark_input* in, cudaStream_t stream) {
   std::vector<std::string> head = split_csv_line(line(0), (char)in->delim);
   if (in->has_header)
     for (auto& h : head)
-      if (!utf8_valid((const uint8_t*)h.data(), (long long)h.size())) fail(ARK_ERR_PROCESS, "Read input failed: Arrow error: Csv error: Encountered invalid UTF-8 data for line 1");
+      if (!utf8_valid((const uint8_t*)h.data(), (long long)h.size())) fail(ARK_ERR_PROCESS, "Read input failed: Arrow error: Csv error: Encountered invalid UTF-8 data for line " + std::to_string(physical_line(in, starts[0], stream)));
   if (in->has_header) in->csv_names = head;
   else for (size_t i = 0; i < head.size(); ++i) in->csv_names.push_back("column_" + std::to_string(i + 1));
   if ((int)in->csv_names.size() > CSV_MAX_COLS) fail(ARK_ERR_UNSUPPORTED, "csv input: more than 32 columns");
   std::vector<int> types(in->csv_names.size(), -1);
   for (int64_t i = in->has_header ? 1 : 0; i < sample_lines; ++i) {
-    const std::string l = line(i);
-    if (l.empty()) continue;
-    std::vector<std::string> f = split_csv_line(l, (char)in->delim);
+    std::vector<std::string> f = split_csv_line(line(i), (char)in->delim);
     for (size_t c = 0; c < types.size() && c < f.size(); ++c) types[c] = csv_infer_type(f[c], types[c]);
   }
   for (auto& t : types) if (t < 0) t = CSV_STR;
@@ -468,8 +492,8 @@ Batch csv_batch(ark_input* in, int64_t l0, int64_t n, cudaStream_t stream) {
   P.data += byte0; P.line_off = (const int32_t*)loff.get(); P.n_rows = n; P.n_cols = nc; P.delim = in->delim;
   std::vector<BufferPtr> vals(nc), valid(nc), slen(nc), ssrc(nc), sraw(nc);
   BufferPtr err = device_alloc(16);
-  ARK_CUDA(cudaMemsetAsync(err.get(), 0, 16, stream));
-  P.error = (int32_t*)err.get();
+  ARK_CUDA(cudaMemsetAsync(err.get(), 0xFF, 16, stream));
+  P.error = (unsigned long long*)err.get();
   for (int c = 0; c < nc; ++c) {
     P.types[c] = in->csv_types[c];
     valid[c] = device_alloc((size_t)std::max<int64_t>(n, 1));
@@ -491,9 +515,12 @@ Batch csv_batch(ark_input* in, int64_t l0, int64_t n, cudaStream_t stream) {
   BufferPtr herr = pinned_alloc(16);
   ARK_CUDA(cudaMemcpyAsync(herr.get(), err.get(), 8, cudaMemcpyDeviceToHost, stream));
   ARK_CUDA(cudaStreamSynchronize(stream));
-  const int32_t ecode = ((int32_t*)herr.get())[0], erow = ((int32_t*)herr.get())[1];
-  if (ecode) {
-    const long long lineno = l0 + erow + 1;
+  const unsigned long long ekey = *(const unsigned long long*)herr.get();
+  if (ekey != ~0ull) {
+    const int ecode = (int)(ekey & 3);
+    ARK_CUDA(cudaMemcpyAsync(herr.get(), (const long long*)in->line_off.get() + l0 + (long long)(ekey >> 2), 8, cudaMemcpyDeviceToHost, stream));
+    ARK_CUDA(cudaStreamSynchronize(stream));
+    const long long lineno = physical_line(in, *(const long long*)herr.get(), stream);
     fail(ARK_ERR_PROCESS, ecode == 2 ? "Read input failed: Arrow error: Csv error: incorrect number of fields for line " + std::to_string(lineno)
                           : ecode == 3 ? "Read input failed: Arrow error: Csv error: Encountered invalid UTF-8 data for line " + std::to_string(lineno)
                                        : "Read input failed: Arrow error: Parser error: Error while parsing value of line " + std::to_string(lineno));
@@ -591,7 +618,7 @@ bool input_next(ark_input* in, Batch& out, cudaStream_t stream) {
     } else {
       b = csv_batch(in, l0, n, stream);
     }
-    if (b.num_rows == 0) continue;  // a run of blank lines
+    if (b.num_rows == 0) continue;  // NDJSON lines that hold only spaces
     if (in->sql) {
       std::vector<Field> fields;
       for (auto& c : b.cols) { Field f = c.field; if (f.format.empty()) f.format = dtype_arrow_format(f.type); fields.push_back(f); }
