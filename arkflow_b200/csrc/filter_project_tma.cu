@@ -785,14 +785,15 @@ __global__ void __launch_bounds__(256, MINB) filter_project_pipe_kernel(const __
 // ================================================================================================
 // filter_project_tile_kernel — the default.  Warp-striped rows (lane l of warp w owns rows 128w + 32j + l: coalesced
 // 8-byte loads and stores, no shared-memory bank conflicts), ONE tile per CTA, a ninth warp that sets up the bulk copy of
-// the tile's string bytes and runs the two-level look-back while the data warps compact the strings.
-// On config 2 (2^24 rows):
+// the tile's string bytes and runs the look-back while the data warps compact the strings.  Default: 2048-row tiles (DT = 512).
+// On config 2 (2^24 rows, H100):
 //   * with the look-back stubbed out the kernel is the data path alone; the look-back adds the time a tile's CTA waits for
 //     the aggregates of the tiles before it (their loads were issued at the same time and some always land late), during
-//     which it holds its slot on the SM without having loads in flight.  5 CTAs per SM (40 registers x 288 threads) do not
-//     cover it, and 7 CTAs at 32 registers spill.  2048-row tiles (DT = 512), a ticket instead of blockIdx, one chain of
-//     tile descriptors instead of the two levels and the persistent pipelined kernel above (its CTAs wait for each other
-//     in a convoy) were all slower.
+//     which it holds its slot on the SM without having loads in flight.  At 40 registers, 2048-row tiles keep 3 x 16 = 48
+//     data warps per SM where 1024-row tiles keep 5 x 8 = 40, and half as many tiles wait on a look-back: 3-4 % faster on
+//     H100 (DESIGN.md §8).  7 CTAs at 32 registers spill.  A ticket instead of blockIdx, one chain of tile descriptors
+//     instead of the two levels, the persistent pipelined kernel above (its CTAs wait for each other in a convoy) and
+//     prefixes resolved per thread-block cluster through DSMEM (DESIGN.md §8) were all slower.
 //   * tried against that wait and dropped: "scout" CTAs that compute the aggregates of a whole group of 32 tiles ahead of
 //     the tiles' own CTAs (one CTA cannot stream a group's inputs fast enough to stay ahead); the look-back warp of every
 //     CTA computing the aggregate of the tile 64-2048 tiles ahead from a bulk copy of its predicate column and offsets,
@@ -803,7 +804,7 @@ __global__ void __launch_bounds__(256, MINB) filter_project_pipe_kernel(const __
 // the cap from __launch_bounds__'s minBlocks (544 threads, 3 blocks → 32 registers and spills instead of the 40 that fit)
 template <int NF, bool VARLEN, int MAXR, int DT>
 __global__ void __launch_bounds__(DT + 32) __maxnreg__(MAXR) filter_project_tile_kernel(const __grid_constant__ TmaParams P) {
-  // warps 0..7: the tile's rows; warp 8: producer (tile id, bulk copy) and look-back — nothing but its own few values is
+  // warps 0..T_WARPS-1: the tile's rows; warp T_WARPS: producer (tile id, bulk copy) and look-back — nothing but its own few values is
   // live there, so the (rare) call into help_publish_aggregate costs the data warps no registers and no spills
   // DT data threads: 256 (1024-row tiles) or 512 (2048-row tiles: half the descriptors on the look-back chain)
   constexpr int T_THREADS = DT, TT = T_THREADS * 4, T_WARPS = T_THREADS / 32, LB_WARP = T_WARPS;
@@ -1293,7 +1294,18 @@ __global__ void __launch_bounds__(DT + 32) filter_project_ring_kernel(const __gr
 
 static std::atomic<double> g_avg_len_hint{12.8};
 void filter_project_tma_note_avg_len(double avg) { if (avg > 0) g_avg_len_hint.store(avg); }
-static int g_fp_threads = [] { const char* e = getenv("ARK_FP_THREADS"); const int v = e ? atoi(e) : 256; return v == 512 || v == 128 ? v : 256; }();
+// implementation: 2 = striped rows, one tile per CTA (default); 0 = persistent pipelined striped kernel; 1 = the r1 kernel
+// (blocked rows, tile = blockIdx); 3 = the persistent ring kernel.  0, 1 and 3 are kept for A/B runs.
+static const int g_fp_impl = [] { const char* e = getenv("ARK_FP_IMPL"); return e ? atoi(e) : 2; }();
+// data threads per CTA (ARK_FP_THREADS = 128 | 256 | 512).  The tile kernel defaults to 512 (2048-row tiles): at 40 registers
+// three 17-warp CTAs fit per SM, 48 data warps against 40 for five 9-warp CTAs, and half the tiles wait on a look-back
+// (DESIGN.md §8).  The other kernels default to 256.
+static const int g_fp_threads = [] {
+  const char* e = getenv("ARK_FP_THREADS");
+  const int v = e ? atoi(e) : 0;
+  if (v == 512 || v == 256 || v == 128) return v;
+  return g_fp_impl == 2 ? 512 : 256;
+}();
 static int g_desc_stride = [] { const char* e = getenv("ARK_FP_DESC_STRIDE"); int v = e ? atoi(e) : 4; return v >= 1 && v <= 16 ? v : 4; }();  // one descriptor per 32-byte sector
 int filter_project_tma_tile_rows() { return g_fp_threads * 4; }
 int filter_project_tma_desc_stride() { return g_desc_stride; }
@@ -1346,8 +1358,8 @@ bool launch_filter_project_tma(int64_t n_rows, const void* pred_in, int n_fixed_
   static const int lb_sleep = [] { const char* e = getenv("ARK_FP_LB_SLEEP"); return e ? atoi(e) : 0; }();
   // the look-back warp sleeps this long before its first poll: the aggregates it needs belong to tiles whose loads were issued
   // at about the same time as its own, and the 60-odd descriptor loads of a poll that finds them missing are wasted L2
-  // requests (measured on 2^24 rows over 0-1500 ns: shortest around 800-1000 ns)
-  static const int lb_delay = [] { const char* e = getenv("ARK_FP_LB_DELAY"); return e ? atoi(e) : 800; }();
+  // requests (measured on 2^24 rows: shortest around 800-1000 ns with 1024-row tiles, 1500 ns with 2048-row tiles, whose loads take longer)
+  static const int lb_delay = [] { const char* e = getenv("ARK_FP_LB_DELAY"); return e ? atoi(e) : g_fp_threads == 512 ? 1500 : 800; }();
   P.lb_sleep = lb_sleep; P.lb_delay = lb_delay;
   // string staging sized from the batch's average string length (+25 %), 2 KB granules, 4..24 KB
   int cap = 0;
@@ -1361,9 +1373,7 @@ bool launch_filter_project_tma(int64_t n_rows, const void* pred_in, int n_fixed_
   P.str_cap = cap;
   P.desc_stride = g_desc_stride;
   const bool v = P.has_varlen;
-  // implementation: 2 = striped rows, one ticketed tile per CTA (default); 0 = persistent pipelined striped kernel;
-  // 1 = the r1 kernel (blocked rows, tile = blockIdx).  0 and 1 are kept for A/B runs.
-  static const int impl = [] { const char* e = getenv("ARK_FP_IMPL"); return e ? atoi(e) : 2; }();
+  const int impl = g_fp_impl;
   if (g_fp_threads == 128 && (impl != 3 || !v)) return false;  // 512-row tiles: the ring kernel only
   if (impl == 3 && v && ticket != nullptr && g_fp_threads <= 256) {
     int nfx = 0;
