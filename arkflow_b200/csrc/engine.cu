@@ -109,13 +109,11 @@ const char* vm_error_text(int e) {
 // ---- fast path: filter_project_tma.cu ------------------------------------------------------------------
 int filter_project_tma_tile_rows();
 int filter_project_tma_max_fixed_out();
-int filter_project_tma_desc_stride();
 size_t filter_project_tma_desc_words(int64_t n_tiles);
 void filter_project_tma_note_avg_len(double avg);
 bool launch_filter_project_tma(int64_t n_rows, const void* pred_in, int n_fixed_out, const void* const* fixed_in, void* const* fixed_out,
                                const int32_t* offsets_in, const uint8_t* data_in, int64_t data_bytes, int32_t* offsets_out, uint8_t* data_out,
-                               int cmp, int is_f64, uint64_t constant, unsigned long long* desc, unsigned int* ticket, long long* totals,
-                               cudaStream_t stream);
+                               int cmp, int is_f64, uint64_t constant, unsigned long long* desc, long long* totals, cudaStream_t stream);
 
 // SELECT <fixed-width cols…> [, <1 var-len col>] WHERE <fixed col> <cmp> <literal>, no NULLs in the used columns.
 static bool try_fast_filter(const Plan& plan, Batch& in, Batch& out, cudaStream_t stream) {
@@ -147,9 +145,8 @@ static bool try_fast_filter(const Plan& plan, Batch& in, Batch& out, cudaStream_
   const Column* vs = varlen_out >= 0 ? &src_col(plan.outputs[varlen_out].src.slot) : nullptr;
   if (vs) { obuf = device_alloc((size_t)(n + 1) * 4 + 16); dbuf = device_alloc((size_t)std::max<int64_t>(varlen_bytes_bound(*vs), 0) + 32); }
   const size_t desc_bytes = filter_project_tma_desc_words(n_tiles) * 8;
-  const size_t scratch_bytes = round_up((int64_t)desc_bytes + 64 + FP_CHANNELS * 8, 256);
-  BufferPtr scratch = device_alloc(scratch_bytes);
-  ARK_CUDA(cudaMemsetAsync(scratch.get(), 0, scratch_bytes, stream));
+  BufferPtr desc = device_alloc(desc_bytes);
+  ARK_CUDA(cudaMemsetAsync(desc.get(), 0, desc_bytes, stream));
   // the kernel's last tile stores the two totals straight into pinned host memory (device-accessible under unified
   // addressing): one stream synchronize, no separate device→host copy on the critical path of every call
   BufferPtr host_res = pinned_alloc(64);
@@ -157,7 +154,7 @@ static bool try_fast_filter(const Plan& plan, Batch& in, Batch& out, cudaStream_
   if (!launch_filter_project_tma(n, src_col(plan.simple.slot).data, (int)fixed_outs.size(), fin, fout, vs ? vs->offsets : nullptr,
                                  vs ? vs->data : nullptr, vs ? vs->data_bytes : 0 /* -1 = unknown */, vs ? (int32_t*)obuf.get() : nullptr,
                                  vs ? (uint8_t*)dbuf.get() : nullptr, plan.simple.cmp, plan.simple.is_f64, plan.simple.constant,
-                                 (unsigned long long*)scratch.get(), (unsigned int*)((char*)scratch.get() + desc_bytes), totals, stream))
+                                 (unsigned long long*)desc.get(), totals, stream))
     return false;
   ARK_CUDA(cudaGetLastError());
   ARK_CUDA(cudaStreamSynchronize(stream));

@@ -1,13 +1,11 @@
 """Every filter + project kernel against the oracle (oracle/sql_oracle.py), at the shapes and values where kernels go wrong.
 
-The fast path `SELECT <≤ 2 Int64/Float64 columns> [, <one Utf8/Binary column>] WHERE <col> <cmp> <literal>` has several
-kernels, each with its own copy of the predicate, ranking, look-back and string staging (DESIGN.md §4.1): the default
-tile kernel (filter_project_tile_kernel), the persistent ring kernel (ARK_FP_IMPL=3), the persistent pipelined kernel
-(ARK_FP_IMPL=0) and the round-1 kernel (ARK_FP_IMPL=1); every other query runs the general filter_project_kernel<PRED, NV>.
-The knobs that pick a kernel are read once per process, so each path runs in a child process: this process builds the
-inputs and the oracle's answers, the child runs the library and writes its results as Arrow IPC together with the kernels
-each call launched.  Every case asserts that the intended kernel ran, or that the path declines the case by design (the
-ring kernel's (NF, NFX) set and shared-memory budget, 512-row tiles without a string output): a silent fallback fails.
+The fast path `SELECT <≤ 2 Int64/Float64 columns> [, <one Utf8/Binary column>] WHERE <col> <cmp> <literal>` runs the
+tile kernel (filter_project_tile_kernel, 2048-row tiles, DESIGN.md §4.1); every other query runs the general
+filter_project_kernel<PRED, NV>.  The tile kernel is run as built and with its look-back forced to help (ARK_FP_DEBUG=4:
+late tiles, a spin limit of 2).  That knob is read once per process, so each path runs in a child process: this process
+builds the inputs and the oracle's answers, the child runs the library and writes its results as Arrow IPC together with
+the kernels each call launched.  Every case asserts that the intended kernel ran: a silent fallback fails.
 
 Survival is decided by construction: the predicate column holds values on the right side of the literal exactly where a
 selection pattern says so (all, none, alternating, one row per tile, runs of empty and full tiles and groups of 32
@@ -29,52 +27,23 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 pytestmark = pytest.mark.gpu
 
 I64_MIN, I64_MAX = -2 ** 63, 2 ** 63 - 1
-TILE, RING, PIPE, R1, GENERAL = ("filter_project_tile_kernel", "filter_project_ring_kernel", "filter_project_pipe_kernel",
-                                 "filter_project_r1_kernel", "filter_project_kernel")
-FAST = (TILE, RING, PIPE, R1)
-KERNELS = ("filter_project_tma_kernel",) + FAST + (GENERAL,)
+TILE, GENERAL = "filter_project_tile_kernel", "filter_project_kernel"
+KERNELS = ("filter_project_tma_kernel", TILE, GENERAL)
 NAN_BITS = np.array([0x7FF8000000000000, 0xFFF8000000000000, 0x7FF0000000000001, 0xFFF0000000000001, 0x7FFFFFFFFFFFFFFF,
                      0xFFFFFFFFFFFFFFFF, 0x7FF4000000000123, 0xFFF400000000ABCD], dtype=np.uint64)
 
 PATHS = {  # name → (environment, kernel it selects, rows per tile)
-    "default": ({}, TILE, 1024),
-    "tiles2048": ({"ARK_FP_THREADS": "512"}, TILE, 2048),
-    "ticket": ({"ARK_FP_TICKET": "1"}, TILE, 1024),
-    "lb_chain": ({"ARK_FP_LB": "1"}, TILE, 1024),
-    "lb_narrow": ({"ARK_FP_LB_WINDOWS": "1"}, TILE, 1024),
-    "maxr32": ({"ARK_FP_MAXR": "32"}, TILE, 1024),
-    "maxr56": ({"ARK_FP_MAXR": "56"}, TILE, 1024),
-    "desc_dense": ({"ARK_FP_DESC_STRIDE": "1"}, TILE, 1024),
-    "small_staging": ({"ARK_FP_CAP_SLACK": "0.25"}, TILE, 1024),
-    "helping": ({"ARK_FP_DEBUG": "4"}, TILE, 1024),
-    "helping_narrow": ({"ARK_FP_DEBUG": "4", "ARK_FP_LB_WINDOWS": "1"}, TILE, 1024),
-    "ring": ({"ARK_FP_IMPL": "3"}, RING, 1024),
-    "ring512": ({"ARK_FP_IMPL": "3", "ARK_FP_THREADS": "128"}, RING, 512),
-    "pipe_minb3": ({"ARK_FP_IMPL": "0", "ARK_FP_MINB": "3"}, PIPE, 1024),
-    "pipe_minb4": ({"ARK_FP_IMPL": "0", "ARK_FP_MINB": "4"}, PIPE, 1024),
-    "pipe_minb5": ({"ARK_FP_IMPL": "0", "ARK_FP_MINB": "5"}, PIPE, 1024),
-    "r1_256": ({"ARK_FP_IMPL": "1"}, R1, 1024),
-    "r1_512": ({"ARK_FP_IMPL": "1", "ARK_FP_THREADS": "512"}, R1, 2048),
+    "default": ({}, TILE, 2048),
+    "helping": ({"ARK_FP_DEBUG": "4"}, TILE, 2048),
 }
 
 
-# ---- staging size and ring budget, as launch_filter_project_tma computes them (csrc/filter_project_tma.cu) -------------
-def str_cap(avg_len, tt, slack=1.0625):
-    """Shared-memory bytes per string buffer: `cap = round_up((int64_t)(avg * TT * slack) + 64, 1024)`, clamped to
-    [4096 (2048 for 512-row tiles), 24 KB per 1024 rows]; avg = referenced string bytes / rows of the batch."""
-    cap = -(-(int(avg_len * tt * slack) + 64) // 1024) * 1024
-    return max(4096 if tt >= 1024 else 2048, min(cap, max(tt // 1024, 1) * 24 * 1024))
-
-
-def ring_takes(nf, nfx, cap, tt):
-    """The ring kernel exists for (NF, NFX) ∈ {(0,0), (1,0), (1,1), (2,1)} and runs when two input and two output stages
-    fit in 112 KB of shared memory."""
-    if (nf, nfx) not in ((0, 0), (1, 0), (1, 1), (2, 1)):
-        return False
-    pred = tt * 8 + 32
-    offs = ((tt + 1) * 4 + 32 + 15) // 16 * 16
-    smem = 2 * (pred + offs + nfx * pred + cap + 32) + 2 * (nf * tt * 8 + tt * 4 + 16 + cap + 32)
-    return smem <= 112 * 1024
+# ---- staging size, as launch_filter_project_tma computes it (csrc/filter_project_tma.cu) ------------------------------
+def str_cap(avg_len, tt):
+    """Shared-memory bytes per string buffer: `cap = round_up((int64_t)(avg * TT * 1.0625) + 64, 1024)`, clamped to
+    [4 KB, 48 KB]; avg = referenced string bytes / rows of the batch."""
+    cap = -(-(int(avg_len * tt * 1.0625) + 64) // 1024) * 1024
+    return max(4096, min(cap, 48 * 1024))
 
 
 # ---- inputs -----------------------------------------------------------------------------------------------------------
@@ -148,7 +117,7 @@ def make_table(n, pattern="s0.5", tt=1024, strings="mixed", seed=0, binary=True)
     return pa.record_batch(cols)
 
 
-def window_table(tt=1024):
+def window_table(tt):
     """Tiles of 12-byte strings, except one tile whose string bytes are exactly str_cap and one with str_cap + 16; every
     tile's bytes are a multiple of 16, so a tile's 16-byte-aligned window is its own bytes.  The first is staged through
     shared memory and fills it to the last byte, the second takes the unstaged path."""
@@ -301,11 +270,10 @@ def _fast_cases(path):
         for name in ("nf1_pred", "nf2", "nf0", "bin_nfx2"):
             _, q, nf, nfx, v = SHAPE[name]
             _case(cases, path, f"str:{strings}", q, nf, nfx, v)
-    if tt == 1024:
-        for name in ("nf1_pred", "nf0", "bin_nf2"):
-            _, q, nf, nfx, v = SHAPE[name]
-            _case(cases, path, "window:1024", q, nf, nfx, v)
-    if path in ("default", "ring", "pipe_minb4"):  # device slices: unaligned data pointers, offsets[0] != 0
+    for name in ("nf1_pred", "nf0", "bin_nf2"):
+        _, q, nf, nfx, v = SHAPE[name]
+        _case(cases, path, f"window:{tt}", q, nf, nfx, v)
+    if path == "default":  # device slices: unaligned data pointers, offsets[0] != 0
         for off in (1, 3, 7, 1237):
             for name in ("nf1_pred", "nf2", "nf0", "nfx2", "str_f"):
                 _, q, nf, nfx, v = SHAPE[name]
@@ -499,36 +467,11 @@ def _first_diff(g, w):
     return None
 
 
-def _string_bytes(col):
-    offs = np.frombuffer(col.buffers()[1], np.int32)[col.offset:col.offset + len(col) + 1]
-    return int(offs[-1]) - int(offs[0])
-
-
-def _expected_kernel(path, c, avg_hint):
-    """The kernel case `c` must run on `path`.  The staging size follows the batch's average string length; a device
-    batch's string extent is not resolved for the fast path, which then sizes from the average selected length of the
-    previous fast-path call in the process (`avg_hint`)."""
-    if c["general"]:
-        return GENERAL
-    _, kernel, tt = PATHS[path]
-    if kernel != RING:
-        return kernel
-    if c["v"]:
-        rb = _sliced(c["table"], c["off"])
-        col = rb.column("bsensor" if "bsensor" in c["query"] else "sensor")
-        avg = avg_hint if c["device"] else _string_bytes(col) / len(col)
-        if ring_takes(c["nf"], c["nfx"], str_cap(avg, tt), tt):
-            return RING
-    # declined by the ring kernel: the one-tile-per-CTA kernel takes it; with 512-row tiles nothing but the general kernel
-    return TILE if tt == 1024 else GENERAL
-
-
 def _run_path(path, tmp, tables_dir, cases, env=None):
     env = PATHS[path][0] if env is None else env
     _write_inputs(tables_dir, cases)
     report = _run_child(str(tmp), tables_dir, cases, env)
     seen = {}
-    avg_hint = 12.8  # filter_project_tma.cu: g_avg_len_hint before the first call
     for c in cases:
         what = (path, c["table"], c["query"], c["off"], c["device"])
         run = report[c["id"]]
@@ -537,12 +480,10 @@ def _run_path(path, tmp, tables_dir, cases, env=None):
         assert want is not None and not run["none"], (what, want, run)
         got = read_result(os.path.join(str(tmp), f"{c['id']}.arrow"), what)
         compare(got, want, what)
-        need = _expected_kernel(path, c, avg_hint)
-        if need != GENERAL and c["v"] and got.num_rows > 0:
-            avg_hint = _string_bytes(got.column([n for n in got.schema.names if "sensor" in n][0])) / got.num_rows
+        need = GENERAL if c["general"] else PATHS[path][1]
         counts = run["counts"]
         assert counts[need] >= 1, (what, need, counts)
-        assert all(counts[k] == 0 for k in FAST + (GENERAL,) if k != need), (what, need, counts)
+        assert all(counts[k] == 0 for k in (TILE, GENERAL) if k != need), (what, need, counts)
         # every fast-path launch is timed under filter_project_tma_kernel as well (the name bench.py reports)
         assert counts["filter_project_tma_kernel"] == (counts[need] if need != GENERAL else 0), (what, counts)
         seen[need] = seen.get(need, 0) + 1
@@ -573,7 +514,7 @@ def test_limit_matches_oracle(gpu, tmp_path, tables_dir):
 
 
 def test_config2_batch_of_2_24_rows(gpu, tmp_path, tables_dir):
-    """One batch of 2^24 + 1 rows on the default path (16 385 tiles, 513 groups), every row and half of them surviving;
+    """One batch of 2^24 + 1 rows on the default path (8 193 tiles, 257 groups), every row and half of them surviving;
     compared with a numpy mask and pc.filter (test_oracle_crosscheck ties pc.filter to the oracle)."""
     cases = []
     for pattern in ("all", "s0.5"):

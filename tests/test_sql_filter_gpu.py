@@ -162,41 +162,13 @@ def test_divide_by_zero_is_a_process_error(gpu):
     check(rb, "SELECT 10 / value FROM flow WHERE value > 0")
 
 
-def test_lookback_helping_path(gpu):
-    """Forward progress without in-order dispatch: with ARK_FP_DEBUG=4 some tiles publish their aggregate late and the
-    look-back of their successors gives up spinning after 2 polls and computes the missing aggregates itself
-    (help_publish_aggregate, csrc/filter_project_tma.cu).  Results must not change.  Run in a subprocess: the knob is
-    read once per process."""
-    import os
-    import subprocess
-    import sys
-
-    code = '''
-import sys
-sys.path.insert(0, %r)
-from arkflow_b200 import _lib as L
-from arkflow_b200.processor import SqlProcessor, MessageBatch, _check
-from oracle.sql_oracle import sql_process
-from oracle.synth import synth_batch
-_check(L.lib().ark_b200_init(0))
-for n, q in ((300_000, "SELECT sensor, value FROM flow WHERE value >= 10"), (257_123, "SELECT timestamp, value FROM flow WHERE value < 7"),
-             (99_999, "SELECT sensor FROM flow WHERE value <> 3")):
-    rb = synth_batch(n, key_space=1000)
-    got = SqlProcessor({"query": q}).process(MessageBatch.new_arrow(rb)).batches[0].record_batch
-    assert got.equals(sql_process(rb, q)), q
-print("HELP_OK")
-''' % os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=300, env=dict(os.environ, ARK_FP_DEBUG="4"))
-    assert r.returncode == 0 and "HELP_OK" in r.stdout, r.stdout[-1500:] + r.stderr[-1500:]
-
-
-@pytest.mark.parametrize("env", [{"ARK_FP_IMPL": "3"}, {"ARK_FP_IMPL": "3", "ARK_FP_THREADS": "128"}, {"ARK_FP_IMPL": "3", "ARK_FP_DEBUG": "4"},
-                                 {"ARK_FP_IMPL": "1"}, {"ARK_FP_IMPL": "1", "ARK_FP_TICKET": "1", "ARK_FP_THREADS": "512"}, {"ARK_FP_THREADS": "512"}])
-def test_alternative_filter_kernels(gpu, env):
-    """The kernels kept next to the default for A/B runs — the persistent ring kernel (ARK_FP_IMPL=3: every input by TMA, store of
-    tile k after the count of tile k+1; also with 512-row tiles and with forced helping), the blocked-row kernel of round 1
-    (ARK_FP_IMPL=1, with and without a ticket) and 2048-row tiles — give the oracle's results too, ragged last tiles, long
-    strings (the unstaged path) and an empty result included.  Subprocess: the knobs are read once per process."""
+@pytest.mark.parametrize("env", [{}, {"ARK_FP_DEBUG": "4"}], ids=["default", "helping"])
+def test_fast_path_in_subprocess(gpu, env):
+    """The fast path's tile kernel as built and with forced helping — forward progress without in-order dispatch: with
+    ARK_FP_DEBUG=4 some tiles publish their aggregate late and the look-back of their successors gives up spinning after 2
+    polls and computes the missing aggregates itself (help_publish_aggregate, csrc/filter_project_tma.cu).  Both give the
+    oracle's results, ragged last tiles, long strings (the unstaged path) and an empty result included.  Subprocess: the
+    knob is read once per process."""
     import os
     import subprocess
     import sys
@@ -212,7 +184,8 @@ from oracle.synth import synth_batch
 _check(L.lib().ark_b200_init(0))
 cases = [(300_000, "SELECT sensor, value FROM flow WHERE value >= 10"), (257_123, "SELECT timestamp, value, sensor FROM flow WHERE value < 7"),
          (99_999, "SELECT sensor FROM flow WHERE value <> 3"), (1, "SELECT sensor, value FROM flow WHERE value >= 0"),
-         (5_000, "SELECT sensor, value FROM flow WHERE value > 1000"), (1_000_003, "SELECT sensor, timestamp FROM flow WHERE value >= 19")]
+         (5_000, "SELECT sensor, value FROM flow WHERE value > 1000"), (1_000_003, "SELECT sensor, timestamp FROM flow WHERE value >= 19"),
+         (257_123, "SELECT timestamp, value FROM flow WHERE value < 7")]
 for n, q in cases:
     rb = synth_batch(n, key_space=1000)
     got = SqlProcessor({"query": q}).process(MessageBatch.new_arrow(rb)).batches[0].record_batch
@@ -222,10 +195,10 @@ long_rb = pa.record_batch({"value": pa.array([i %% 20 for i in range(40_000)], p
 q = "SELECT sensor, value FROM flow WHERE value >= 10"
 got = SqlProcessor({"query": q}).process(MessageBatch.new_arrow(long_rb)).batches[0].record_batch
 assert got.equals(sql_process(long_rb, q)), "long strings"
-print("ALT_OK")
+print("FAST_OK")
 ''' % os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=300, env=dict(os.environ, **env))
-    assert r.returncode == 0 and "ALT_OK" in r.stdout, r.stdout[-1500:] + r.stderr[-1500:]
+    assert r.returncode == 0 and "FAST_OK" in r.stdout, r.stdout[-1500:] + r.stderr[-1500:]
 
 
 def test_min_over_minus_one_overflows_for_div_and_mod(gpu):
@@ -303,12 +276,12 @@ print("SLICES_OK")
 ''' % os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-@pytest.mark.parametrize("env", [{}, {"ARK_FP_IMPL": "3"}])
+@pytest.mark.parametrize("env", [{}, {"ARK_FP_DEBUG": "4"}])
 def test_device_sliced_inputs(gpu, env):
     """Device batches whose columns are Arrow slices, as a producer that slices device batches hands them over: Int64 data
     8 bytes past a 16-byte boundary, offsets 4-aligned with offsets[0] != 0, validity and Boolean bits that start inside a
-    byte.  The default tile kernel and the ring kernel (ARK_FP_IMPL=3, every input staged by TMA).  Subprocess: the knob is
-    read once per process."""
+    byte.  The fast path as built and with forced helping (ARK_FP_DEBUG=4), whose look-back then reads the sliced predicate
+    column and offsets itself.  Subprocess: the knob is read once per process."""
     import subprocess
     import sys
 
