@@ -88,6 +88,19 @@ const std::string& protobuf_to_arrow_value_field(const Processor& p);
 Batch protobuf_to_arrow_device(const Processor& proc, Batch& in, cudaStream_t stream);
 std::unique_ptr<Processor> make_arrow_to_protobuf(const char* config_json);
 Batch arrow_to_protobuf_device(const Processor& proc, Batch& in, cudaStream_t stream);
+// protobuf.cu: exclusive scan of n + 1 int32 lengths into a column's offsets; the guard that fails with Process when the
+// lengths add up past a Binary / Utf8 column's 2 GiB (checked exactly only when `bound` does not rule it out); the copy
+// of each row's span of `data` into the column's bytes
+BufferPtr pb_scan(const int32_t* lens, int64_t n, cudaStream_t stream);
+void pb_check_total(const int32_t* lens, int64_t n, int64_t bound, const std::string& what, cudaStream_t stream);
+void launch_span_copy(const uint8_t* data, const long long* src, const int32_t* offsets, int64_t n_rows, uint8_t* out, cudaStream_t stream);
+// avro.cu: the `file` input's Avro object container files
+struct AvroFile;
+std::shared_ptr<AvroFile> avro_open(const std::string& path);  // header, schema and codec (nullptr: cannot open)
+void avro_scan(AvroFile& f, const uint8_t* p, size_t n, int64_t base);  // the block table, from the file's bytes in order
+void avro_scan_end(AvroFile& f);
+int64_t avro_rows(const AvroFile& f);
+Batch avro_batch(AvroFile& f, const BufferPtr& file_dev, int64_t r0, int64_t n, cudaStream_t stream);
 Batch concat_device(std::vector<Batch>& ins, cudaStream_t stream);
 Batch synth_batch(int64_t n, int64_t row0, uint64_t seed, int value_kind, int64_t key_space, cudaStream_t stream);
 

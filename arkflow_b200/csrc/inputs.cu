@@ -7,11 +7,13 @@
 //               immutable, so here the replicated payload column is built ONCE in HBM (replicate kernel) and every
 //               read() hands out another reference to it — BASELINE configs[4]'s "100 M msg/s generate input" costs
 //               no memory traffic at all until a processor reads the messages.
-//   file      ← crates/arkflow-plugin/src/input/file.rs:395-455 (`input_type: {type: json | csv, path}`, optional
-//               `query`): the file's bytes go to HBM once; line starts are found by a newline-index kernel, NDJSON
-//               lines are decoded by the json_to_arrow kernels (csrc/json.cu), CSV rows by csv_parse_kernel; the
-//               optional query runs through the sql processor.  Parquet / Avro / Arrow IPC and remote object stores
-//               are not read here (ARK_ERR_UNSUPPORTED; SURVEY.md §8(f) rank 4 names CSV / JSON first).
+//   file      ← crates/arkflow-plugin/src/input/file.rs:395-455 (`input_type: {type: json | csv | avro, path}`,
+//               optional `query`): the file's bytes go to HBM once; line starts are found by a newline-index kernel,
+//               NDJSON lines are decoded by the json_to_arrow kernels (csrc/json.cu), CSV rows by csv_parse_kernel,
+//               Avro object container files (codecs null and snappy) by the kernels of csrc/avro.cu, whose block table
+//               is built on the host while the upload's chunks pass; the optional query runs through the sql
+//               processor.  Parquet / Arrow IPC, the Avro codecs deflate / zstandard / bzip2 / xz and remote object
+//               stores are not read here (ARK_ERR_UNSUPPORTED).
 //               The NDJSON schema is merged over the first 1000 records and fixed for the file, as DataFusion does.
 //               Deviations from DataFusion's readers: CSV types come from the first 1000 records with the
 //               types Int64 / Float64 / Boolean / Utf8 (dates stay strings), quoted CSV fields may not contain line
@@ -32,6 +34,8 @@
 
 #include <chrono>
 #include <cstdio>
+#include <exception>
+#include <functional>
 #include <thread>
 
 #include <thrust/iterator/counting_iterator.h>
@@ -259,7 +263,7 @@ unsigned grid_of(long long n, int threads = 256) { return (unsigned)std::max<lon
 }  // namespace
 
 struct ark_input {
-  enum Kind { Generate, FileJson, FileCsv } kind = Generate;
+  enum Kind { Generate, FileJson, FileCsv, FileAvro } kind = Generate;
   std::mutex mu;
   // generate
   std::string context;
@@ -274,7 +278,7 @@ struct ark_input {
   BufferPtr file_dev;       // the file's bytes in HBM
   int64_t file_bytes = 0;
   BufferPtr line_off;       // int64 starts of the lines that are not empty (+ file end) on the device
-  int64_t n_lines = 0, next_line = 0, rows_per_batch = 1 << 22;
+  int64_t n_lines = 0, next_line = 0, rows_per_batch = 1 << 22;  // Avro: records, not lines
   std::unique_ptr<Processor> decoder;
   std::unique_ptr<SqlProcessor> sql;
   // csv
@@ -282,6 +286,8 @@ struct ark_input {
   std::vector<int> csv_types;
   int delim = ',';
   bool has_header = true;
+  // avro
+  std::shared_ptr<AvroFile> avro;  // header, schema and block table
 };
 
 namespace {
@@ -311,7 +317,10 @@ Batch generate_batch(ark_input* in, cudaStream_t stream) {
   return b;
 }
 
-void file_connect(ark_input* in, cudaStream_t stream) {
+// `visit`, when given, sees the file's bytes in order as they pass through the pinned chunks: (bytes, count, file offset)
+using ChunkVisitor = std::function<void(const uint8_t*, size_t, int64_t)>;
+
+void file_connect(ark_input* in, cudaStream_t stream, const ChunkVisitor* visit = nullptr) {
   struct stat st;
   if (stat(in->path.c_str(), &st) != 0) fail(ARK_ERR_PROCESS, "Read input failed: Object at location " + in->path + " not found");
   const int64_t n = (int64_t)st.st_size;
@@ -327,12 +336,16 @@ void file_connect(ark_input* in, cudaStream_t stream) {
   int64_t done = 0;
   int turn = 0;
   bool io_error = false;
+  std::exception_ptr visit_error;
   while (done < n) {
     uint8_t* slot = (uint8_t*)stage.get() + (size_t)turn * CH;
     if (used[turn]) ARK_CUDA(cudaEventSynchronize(ev[turn]));
     const size_t want = (size_t)std::min<int64_t>((int64_t)CH, n - done);
     const size_t got = fread(slot, 1, want, f);
     if (got == 0) { io_error = true; break; }
+    if (visit) {
+      try { (*visit)(slot, got, done); } catch (...) { visit_error = std::current_exception(); break; }
+    }
     ARK_CUDA(cudaMemcpyAsync((uint8_t*)in->file_dev.get() + done, slot, got, cudaMemcpyHostToDevice, stream));
     ARK_CUDA(cudaEventRecord(ev[turn], stream));
     used[turn] = true;
@@ -343,7 +356,9 @@ void file_connect(ark_input* in, cudaStream_t stream) {
   ARK_CUDA(cudaStreamSynchronize(stream));
   for (auto& e : ev) cudaEventDestroy(e);
   if (io_error) fail(ARK_ERR_PROCESS, "Read input failed: short read on " + in->path);
+  if (visit_error) std::rethrow_exception(visit_error);
   in->file_bytes = n;
+  if (in->kind == ark_input::FileAvro) return;  // records are found per batch by avro_index_kernel
   // line starts
   if (n == 0) { in->n_lines = 0; return; }
   BufferPtr flags = device_alloc((size_t)n);
@@ -608,7 +623,9 @@ bool input_next(ark_input* in, Batch& out, cudaStream_t stream) {
     const int64_t n = std::min<int64_t>(in->rows_per_batch, in->n_lines - l0);
     in->next_line += n;
     Batch b;
-    if (in->kind == ark_input::FileJson) {
+    if (in->kind == ark_input::FileAvro) {
+      b = avro_batch(*in->avro, in->file_dev, l0, n, stream);
+    } else if (in->kind == ark_input::FileJson) {
       BufferPtr h = pinned_alloc(32);
       ARK_CUDA(cudaMemcpyAsync(h.get(), (const long long*)in->line_off.get() + l0, 8, cudaMemcpyDeviceToHost, stream));
       ARK_CUDA(cudaMemcpyAsync((char*)h.get() + 8, (const long long*)in->line_off.get() + l0 + n, 8, cudaMemcpyDeviceToHost, stream));
@@ -675,8 +692,9 @@ int ark_input_create(const char* type, const char* config_json, ark_input_t** ou
       if (!ty || ty->kind != JsonValue::String) fail(ARK_ERR_SERIALIZATION, "missing field `type` (InputType)");
       if (ty->str == "json") in->kind = ark_input::FileJson;
       else if (ty->str == "csv") in->kind = ark_input::FileCsv;
-      else if (ty->str == "parquet" || ty->str == "avro" || ty->str == "arrow")
-        fail(ARK_ERR_UNSUPPORTED, "file input: " + ty->str + " files are not decoded on the GPU (json and csv are)");
+      else if (ty->str == "avro") in->kind = ark_input::FileAvro;
+      else if (ty->str == "parquet" || ty->str == "arrow")
+        fail(ARK_ERR_UNSUPPORTED, "file input: " + ty->str + " files are not decoded on the GPU (json, csv and avro are)");
       else fail(ARK_ERR_SERIALIZATION, "unknown variant `" + ty->str + "`, expected one of `avro`, `arrow`, `json`, `csv`, `parquet`");
       const JsonValue* p = it->get("path");
       if (!p || p->kind != JsonValue::String) fail(ARK_ERR_SERIALIZATION, "missing field `path`");
@@ -711,6 +729,20 @@ int ark_input_connect(ark_input_t* in) {
     if (in->kind == ark_input::Generate) return;  // generate.rs:62-64
     std::lock_guard<std::mutex> l(in->mu);
     if (in->connected) return;
+    if (in->kind == ark_input::FileAvro) {
+      // the header (schema and codec, whose errors need no device) first, then the block table during the upload
+      std::shared_ptr<AvroFile> av = avro_open(in->path);
+      StreamLease lease;
+      if (!av) { file_connect(in, lease.s); fail(ARK_ERR_PROCESS, "Read input failed: cannot open " + in->path); }
+      const ChunkVisitor visit = [&](const uint8_t* p, size_t n, int64_t base) { avro_scan(*av, p, n, base); };
+      file_connect(in, lease.s, &visit);
+      avro_scan_end(*av);
+      in->avro = av;
+      in->n_lines = avro_rows(*av);
+      in->next_line = 0;
+      in->connected = true;
+      return;
+    }
     StreamLease lease;
     file_connect(in, lease.s);
     if (in->kind == ark_input::FileCsv) csv_prepare(in, lease.s);

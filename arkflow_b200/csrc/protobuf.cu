@@ -386,6 +386,8 @@ __global__ void protobuf_sum64_kernel(const int32_t* lens, int64_t n, unsigned l
   if ((threadIdx.x & 31) == 0) atomicAdd(total, (unsigned long long)acc);
 }
 
+}  // namespace
+
 // The offsets of a Binary / Utf8 column are int32, and so is pb_scan: when lengths add up to 2^31 or more the scan wraps,
 // and once it wraps past 2^32 its last entry looks valid again while earlier offsets point outside the allocation.  When
 // the host's bound on the total (`bound`) does not rule that out, the total is summed exactly first (one more launch and
@@ -415,6 +417,15 @@ BufferPtr pb_scan(const int32_t* lens, int64_t n, cudaStream_t stream) {
   cub::DeviceScan::ExclusiveSum(tmp.get(), tb, lens, (int32_t*)offs.get(), (int)(n + 1), stream);
   return offs;
 }
+
+// string / bytes column bytes from spans of `data`: row r = data[src[r] .. src[r] + offsets[r+1] - offsets[r])
+void launch_span_copy(const uint8_t* data, const long long* src, const int32_t* offsets, int64_t n_rows, uint8_t* out, cudaStream_t stream) {
+  if (n_rows == 0) return;
+  KernelTimer t("protobuf_strings_kernel", stream);
+  protobuf_strings_kernel<<<(unsigned)ceil_div(n_rows, 256), 256, 0, stream>>>(data, nullptr, src, offsets, n_rows, out);
+}
+
+namespace {
 
 // ---- configuration ----------------------------------------------------------------------------------------------
 std::vector<std::string> string_list(const JsonValue& v, const char* key) {

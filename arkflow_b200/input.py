@@ -2,7 +2,7 @@
 
     trait Input { connect, read, close }   → class Input          (core/input/mod.rs)
     GenerateInput                          → class GenerateInput  (plugin/input/generate.rs:26-96)
-    FileInput (json / csv)                 → class FileInput      (plugin/input/file.rs:395-455)
+    FileInput (json / csv / avro)          → class FileInput      (plugin/input/file.rs:395-455)
     InputConfig::build                     → build_input(cfg)
 
 read() returns (MessageBatch, NoopAck) like the reference; read_device() leaves the batch in HBM.  End of input is
@@ -63,7 +63,14 @@ class GenerateInput(Input):
 
 
 class FileInput(Input):
-    """`type: file` {input_type: {type: json | csv, path}, query?: {query, table?}, batch_size?}."""
+    """`type: file` {input_type: {type: json | csv | avro, path}, query?: {query, table?}, batch_size?}.
+
+    `avro`: object container files with codec null or snappy, decoded on the GPU.  The top-level record's fields may be
+    null, boolean, int, long, float, double, bytes or string, or a [null, T] / [T, null] union of one of these: Arrow
+    Null, Boolean, Int32, Int64, Float32, Float64, Binary, Utf8, nullable only for unions.  Other schemas and codecs
+    raise Unsupported from connect(); malformed data raises Process naming the first failing record and its block's
+    file offset (structural damage already from connect()).  SQL `query` over Int32 / Float32 columns is Unsupported.
+    """
 
     TYPE = "file"
 
