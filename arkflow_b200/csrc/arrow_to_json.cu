@@ -39,20 +39,48 @@ struct AjParams {
   AjCol cols[AJ_MAX_COLS];
 };
 
+// kCount: the measure pass, which counts in unsigned 32 bits and saturates at AJ_PAST_INT32 = 2^31.  One Utf8 value alone
+// can pass 2^31 (768 MiB of control characters is 4.5 GiB of JSON, which an int would wrap back to a positive length), so
+// string values are added saturated; everything else in a row (keys, numbers, Booleans, braces) adds at most
+// 2 + 16 * (72 + 1 + 24) bytes, which cannot carry a saturated count past 2^32.  The write pass runs only once the total is
+// known to fit int32, so it keeps int offsets.
+constexpr unsigned AJ_PAST_INT32 = 1u << 31;
+template <bool kCount>
 struct Sink {
-  uint8_t* p;   // nullptr ⇒ counting only
-  int n;
-  __device__ __forceinline__ void put(uint8_t c) { if (p) p[n] = c; ++n; }
+  uint8_t* p;  // unused when counting
+  typename std::conditional<kCount, unsigned, int>::type n;
+  static constexpr bool kCounting = kCount;
+  __device__ __forceinline__ void put(uint8_t c) { if (!kCount) p[n] = c; ++n; }
+  __device__ __forceinline__ void add_saturated(unsigned k) { n = n >= AJ_PAST_INT32 || k >= AJ_PAST_INT32 - n ? max(n, AJ_PAST_INT32) : n + k; }
 };
 
-__device__ void put_u64(Sink& s, unsigned long long v) {
+// Output bytes of one Utf8 value (quotes included) as put_json_string writes it, saturated at AJ_PAST_INT32.  The escapes
+// are counted over 2^28 input bytes at a time (6 output bytes each at most), so no partial count wraps.
+__device__ unsigned json_string_bytes(const uint8_t* p, int len) {
+  unsigned total = 2u + (unsigned)len;
+  for (int i0 = 0; i0 < len && total < AJ_PAST_INT32; i0 += min(len - i0, 1 << 28)) {
+    const int i1 = i0 + min(len - i0, 1 << 28);
+    unsigned extra = 0;
+    for (int i = i0; i < i1; ++i) {
+      const uint8_t c = p[i];
+      if (c == '"' || c == '\\') extra += 1;
+      else if (c < 0x20) extra += (c == '\b' || c == '\f' || c == '\n' || c == '\r' || c == '\t') ? 1 : 5;
+    }
+    total = extra >= AJ_PAST_INT32 - total ? AJ_PAST_INT32 : total + extra;
+  }
+  return min(total, AJ_PAST_INT32);
+}
+
+template <typename S>
+__device__ void put_u64(S& s, unsigned long long v) {
   char buf[20];
   int k = 0;
   do { buf[k++] = (char)('0' + v % 10); v /= 10; } while (v);
   while (k) s.put((uint8_t)buf[--k]);
 }
 
-__device__ void put_i64(Sink& s, long long v) {
+template <typename S>
+__device__ void put_i64(S& s, long long v) {
   if (v < 0) { s.put('-'); put_u64(s, 0ull - (unsigned long long)v); }
   else put_u64(s, (unsigned long long)v);
 }
@@ -148,7 +176,8 @@ __device__ void d2d(unsigned long long bits, unsigned long long* digits, int* ex
   *digits = out; *exp10 = e10 + removed;
 }
 
-__device__ void put_f64(Sink& s, unsigned long long bits) {
+template <typename S>
+__device__ void put_f64(S& s, unsigned long long bits) {
   const unsigned long long mag = bits & 0x7FFFFFFFFFFFFFFFull;
   if ((mag >> 52) == 0x7FF) { s.put('n'); s.put('u'); s.put('l'); s.put('l'); return; }  // NaN / inf
   if (bits >> 63) s.put('-');
@@ -181,7 +210,9 @@ __device__ void put_f64(Sink& s, unsigned long long bits) {
   }
 }
 
-__device__ void put_json_string(Sink& s, const uint8_t* p, int len) {
+template <typename S>
+__device__ void put_json_string(S& s, const uint8_t* p, int len) {
+  if (S::kCounting) { s.add_saturated(json_string_bytes(p, len)); return; }
   const char* hex = "0123456789abcdef";
   s.put('"');
   for (int i = 0; i < len; ++i) {
@@ -199,15 +230,19 @@ __device__ void put_json_string(Sink& s, const uint8_t* p, int len) {
   s.put('"');
 }
 
-__device__ void put_hex(Sink& s, const uint8_t* p, int len) {
+template <typename S>
+__device__ void put_hex(S& s, const uint8_t* p, int len) {
+  if (S::kCounting) { s.add_saturated(len >= (1 << 30) ? AJ_PAST_INT32 : 2u + 2u * (unsigned)len); return; }
   const char* hex = "0123456789abcdef";
   s.put('"');
   for (int i = 0; i < len; ++i) { s.put(hex[p[i] >> 4]); s.put(hex[p[i] & 15]); }
   s.put('"');
 }
 
-__device__ int emit_row(const AjParams& P, int64_t row, uint8_t* out) {
-  Sink s{out, 0};
+// the row's bytes (the measure pass) or the row written at `out` (the write pass)
+template <bool kCount>
+__device__ unsigned emit_row(const AjParams& P, int64_t row, uint8_t* out) {
+  Sink<kCount> s{out, 0};
   s.put('{');
   bool first = true;
   for (int c = 0; c < P.n_cols; ++c) {
@@ -233,12 +268,15 @@ __device__ int emit_row(const AjParams& P, int64_t row, uint8_t* out) {
     }
   }
   s.put('}');
-  return s.n;
+  return (unsigned)s.n;
 }
 
 __global__ void arrow_to_json_measure_kernel(const __grid_constant__ AjParams P, int32_t* lens) {
   const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (r < P.n_rows) lens[r] = emit_row(P, r, nullptr);
+  if (r < P.n_rows) {
+    const unsigned len = emit_row<true>(P, r, nullptr);
+    lens[r] = len < AJ_PAST_INT32 ? (int32_t)len : -1;  // a row past 2^31 - 1 bytes: pb_check_total counts it as too long
+  }
 }
 // The lines of one CTA's rows are contiguous in the output: each thread formats its row into a shared-memory
 // image of that range, which then leaves with 16-byte stores (byte-wise stores at a ~65-byte stride straight
@@ -252,12 +290,12 @@ __global__ void __launch_bounds__(AJ_THREADS) arrow_to_json_write_kernel(const _
   const int64_t r = r0 + threadIdx.x;
   const int32_t bb = offsets[r0];
   const int tb = offsets[r0 + rows] - bb;
-  if (tb + 16 > stage_bytes) {  // long rows: format straight into global memory
-    if (r < P.n_rows) emit_row(P, r, out + offsets[r]);
+  if (tb > stage_bytes - 16) {  // long rows: format straight into global memory (tb + 16 overflows near 2^31)
+    if (r < P.n_rows) emit_row<false>(P, r, out + offsets[r]);
     return;
   }
   const int mis = stage_misalignment(out + bb);
-  if (r < P.n_rows) emit_row(P, r, aj_stage + mis + (offsets[r] - bb));
+  if (r < P.n_rows) emit_row<false>(P, r, aj_stage + mis + (offsets[r] - bb));
   __syncthreads();
   stage_store(out + bb, aj_stage, mis, tb, threadIdx.x, AJ_THREADS);
 }
@@ -314,6 +352,10 @@ Batch arrow_to_json_device(const Processor& proc, Batch& in, cudaStream_t stream
   AjParams P;
   memset(&P, 0, sizeof P);
   P.n_rows = n;
+  // A bound on the output bytes: per row the braces, each column's key and comma and its widest value ("-9223372036854775808",
+  // "-1.2345678901234567e-308", "false", a string's quotes); a Utf8 byte becomes at most 6 ("\u00xx"), a Binary byte 2.
+  // While it stays below 2^31 the exact 64-bit sum in pb_check_total is skipped.
+  int64_t row_bound = 2, var_bound = 0;
   for (auto& c : in.cols) {
     if (!c.present && c.field.format != "n") fail(ARK_ERR_UNSUPPORTED, "arrow_to_json: column '" + c.field.name + "' has Arrow type '" + c.field.format + "'");
     if (c.field.format == "n") continue;  // Null-typed column: never emitted
@@ -325,8 +367,13 @@ Batch arrow_to_json_device(const Processor& proc, Batch& in, cudaStream_t stream
     a.dtype = (int)c.field.type; a.key_len = (int)key.size();
     memcpy(a.key, key.data(), key.size());
     a.view = c.view();
+    const DType t = c.field.type;
+    row_bound += a.key_len + 1 + (t == DType::Int64 ? 20 : t == DType::Float64 ? 24 : t == DType::Bool ? 5 : 2);
+    if (t == DType::Utf8 || t == DType::Binary)
+      var_bound = c.data_bytes < 0 || var_bound < 0 ? -1 : var_bound + (t == DType::Utf8 ? 6 : 2) * c.data_bytes;
   }
   if (ap.has_include && P.n_cols == 0 && n > 0) fail_filtered_to_no_columns();
+  const int64_t bound = var_bound < 0 ? -1 : var_bound + n * row_bound;
   BufferPtr lens = device_alloc((size_t)(n + 1) * 4), offs = device_alloc((size_t)(n + 1) * 4);
   ARK_CUDA(cudaMemsetAsync(lens.get(), 0, (size_t)(n + 1) * 4, stream));
   const unsigned grid = (unsigned)std::max<int64_t>(1, ceil_div(n, 128));
@@ -334,6 +381,8 @@ Batch arrow_to_json_device(const Processor& proc, Batch& in, cudaStream_t stream
     KernelTimer t("arrow_to_json_measure_kernel", stream);
     arrow_to_json_measure_kernel<<<grid, 128, 0, stream>>>(P, (int32_t*)lens.get());
   }
+  // the int32 scan below wraps past 2^31 - 1 (and past 2^32 looks valid again): an output that does not fit fails first
+  pb_check_total((const int32_t*)lens.get(), n, bound, "Arrow JSON Serialization error: arrow_to_json output", stream);
   size_t tb = 0;
   cub::DeviceScan::ExclusiveSum(nullptr, tb, (int32_t*)lens.get(), (int32_t*)offs.get(), (int)(n + 1), stream);
   BufferPtr tmp = device_alloc(tb + 16);
@@ -343,7 +392,6 @@ Batch arrow_to_json_device(const Processor& proc, Batch& in, cudaStream_t stream
   ARK_CUDA(cudaMemcpyAsync(h.get(), (int32_t*)offs.get() + n, 4, cudaMemcpyDeviceToHost, stream));
   ARK_CUDA(cudaStreamSynchronize(stream));
   const int32_t total = *(int32_t*)h.get();
-  if (total < 0) fail(ARK_ERR_PROCESS, "Arrow JSON Serialization error: output exceeds 2 GiB");
   BufferPtr bytes = device_alloc((size_t)total + 16);
   if (n) {
     KernelTimer t("arrow_to_json_write_kernel", stream);

@@ -298,16 +298,23 @@ struct PbEncParams {
   PbEncCol cols[PB_MAX_FIELDS];  // ascending field number
 };
 
+// kCount: the measure pass.  Keys and scalar values (at most 64 * 15 bytes) are counted in `n`, string / bytes payloads in
+// 64 bits in `wide`: three 1.5 GiB `bytes` fields make 4.5 GiB, which an int would wrap back to a positive length.  The
+// write pass runs only once the total fits int32, so it keeps int offsets.
+template <bool kCount>
 struct Sink {
-  uint8_t* p;  // nullptr ⇒ counting only
+  uint8_t* p;      // unused when counting
   int n;
-  __device__ __forceinline__ void put(uint8_t c) { if (p) p[n] = c; ++n; }
+  long long wide;  // counting only
+  __device__ __forceinline__ void put(uint8_t c) { if (!kCount) p[n] = c; ++n; }
   __device__ __forceinline__ void varint(unsigned long long v) { while (v >= 0x80) { put((uint8_t)(v | 0x80)); v >>= 7; } put((uint8_t)v); }
   __device__ __forceinline__ void le(unsigned long long v, int w) { for (int b = 0; b < w; ++b) put((uint8_t)(v >> (8 * b))); }
 };
 
-__device__ __forceinline__ int pb_emit_row(const PbEncParams& P, int64_t row, uint8_t* out) {
-  Sink s{out, 0};
+// the message's bytes (the measure pass) or the message written at `out` (the write pass)
+template <bool kCount>
+__device__ __forceinline__ long long pb_emit_row(const PbEncParams& P, int64_t row, uint8_t* out) {
+  Sink<kCount> s{out, 0, 0};
   for (int c = 0; c < P.n_cols; ++c) {
     const PbEncCol& col = P.cols[c];
     const ColView& v = col.view;
@@ -317,6 +324,7 @@ __device__ __forceinline__ int pb_emit_row(const PbEncParams& P, int64_t row, ui
       if (len == 0 && !col.always) continue;
       for (int b = 0; b < col.key_len; ++b) s.put(col.key[b]);
       s.varint((unsigned)len);
+      if (kCount) { s.wide += len; continue; }
       const uint8_t* src = (const uint8_t*)v.data + o0;
       for (int b = 0; b < len; ++b) s.put(src[b]);
       continue;
@@ -348,12 +356,15 @@ __device__ __forceinline__ int pb_emit_row(const PbEncParams& P, int64_t row, ui
       default: s.varint(raw); break;  // int64, uint64, uint32, bool
     }
   }
-  return s.n;
+  return s.n + s.wide;
 }
 
 __global__ void protobuf_encode_measure_kernel(const __grid_constant__ PbEncParams P, int32_t* lens) {
   const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (r < P.n_rows) lens[r] = pb_emit_row(P, r, nullptr);
+  if (r < P.n_rows) {
+    const long long len = pb_emit_row<true>(P, r, nullptr);
+    lens[r] = len <= INT32_MAX ? (int32_t)len : -1;  // a message past 2^31 - 1 bytes: pb_check_total counts it as too long
+  }
 }
 
 // The messages of one CTA's rows are contiguous in the output: each thread encodes its row into a shared-memory image of
@@ -367,12 +378,12 @@ __global__ void __launch_bounds__(PB_THREADS, 8) protobuf_encode_write_kernel(co
   const int64_t r = r0 + threadIdx.x;
   const int32_t bb = offsets[r0];
   const int tb = offsets[r0 + rows] - bb;
-  if (tb + 16 > stage_bytes) {  // long rows: encode straight into global memory
-    if (r < P.n_rows) pb_emit_row(P, r, out + offsets[r]);
+  if (tb > stage_bytes - 16) {  // long rows: encode straight into global memory (tb + 16 overflows near 2^31)
+    if (r < P.n_rows) pb_emit_row<false>(P, r, out + offsets[r]);
     return;
   }
   const int mis = stage_misalignment(out + bb);
-  if (r < P.n_rows) pb_emit_row(P, r, pe_stage + mis + (offsets[r] - bb));
+  if (r < P.n_rows) pb_emit_row<false>(P, r, pe_stage + mis + (offsets[r] - bb));
   __syncthreads();
   stage_store(out + bb, pe_stage, mis, tb, threadIdx.x, PB_THREADS);
 }

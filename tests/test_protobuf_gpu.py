@@ -10,7 +10,7 @@ import numpy as np
 import pyarrow as pa
 import pytest
 
-from arkflow_b200.arrow_ffi import DeviceBatch
+from arkflow_b200.arrow_ffi import DeviceBatch, DeviceColumn
 from arkflow_b200.processor import (ArkError, ArrowToProtobufProcessor, JsonToArrowProcessor, MessageBatch, Pipeline,
                                     ProtobufToArrowProcessor, SqlProcessor)
 from oracle import protobuf_oracle as O
@@ -470,4 +470,62 @@ def test_string_column_beyond_int32_offsets_is_an_error(gpu, tmp_path, rows):
     assert decode(dec, [b"\x10\x07"] * 3).to_pydict() == {"s": [big] * 3, "i": [7] * 3}
     with pytest.raises(ArkError) as e:
         decode(dec, [b""] * rows)
+    assert e.value.kind == "Process" and "2 GiB" in e.value.message, e.value.message
+
+
+def _pattern_bytes(n):
+    """n bytes of (i % 251) on the device, built 256 MiB at a time."""
+    import torch
+
+    t = torch.empty(n, dtype=torch.uint8, device="cuda")
+    step = 1 << 28
+    for i0 in range(0, n, step):
+        t[i0:i0 + step] = (torch.arange(i0, min(i0 + step, n), device="cuda", dtype=torch.int64) % 251).to(torch.uint8)
+    return t
+
+
+def _device_bytes_column(name, data, length):
+    import torch
+
+    return DeviceColumn(name, "binary", 1, data, torch.tensor([0, length], dtype=torch.int32, device="cuda"), None, 0, False)
+
+
+def test_message_of_2gib_minus_one_bytes(gpu, tmp_path):
+    # one `bytes` field of 2^31 - 7 bytes: key (1) + length varint (5) + payload = 2^31 - 1 bytes, the largest message a
+    # Binary column holds.  Its one CTA takes the direct path: the staging test (tb > stage - 16) holds, where tb + 16
+    # would have overflowed int32 and sent 2 GiB through a 44 KiB shared-memory window.
+    import torch
+
+    L = 2 ** 31 - 7
+    assert 1 + 5 + L == 2 ** 31 - 1 and L >> 28 and not L >> 35  # a 5-byte varint
+    _, enc = processors(tmp_path, [PbField("b", 1, "bytes")])
+    data = _pattern_bytes(L)
+    out = enc.process_device(DeviceBatch([_device_bytes_column("b", data, L)], 1))
+    v = out.columns[-1]
+    assert v.name == "__value__" and v.offsets.cpu().tolist() == [0, 2 ** 31 - 1]
+    got = v.data.tensor()
+    assert got.numel() == 2 ** 31 - 1
+    head = bytes(got[:6].cpu().numpy())
+    assert head == b"\x0a" + bytes([(L >> (7 * k)) & 0x7F | (0x80 if k < 4 else 0) for k in range(5)]), head
+    step = 1 << 28
+    for i0 in range(0, L, step):
+        assert torch.equal(got[6 + i0:6 + min(i0 + step, L)], data[i0:i0 + step]), i0
+    del got
+    out.close()
+
+
+def test_message_of_three_1_5gib_bytes_fields_is_an_error(gpu, tmp_path):
+    # three `bytes` fields of 1.5 GiB each over one device buffer: 4.5 GiB + 18 in one message, which an int32 row length
+    # wraps back to a positive 0.5 GiB; the exact 64-bit count must see it and fail before anything is written
+    import torch
+
+    L = 3 << 29
+    msg = 3 * (1 + 5 + L)
+    assert 2 ** 32 < msg and 0 < msg % 2 ** 32 < 2 ** 31
+    fields = [PbField("b1", 1, "bytes"), PbField("b2", 2, "bytes"), PbField("b3", 3, "bytes")]
+    _, enc = processors(tmp_path, fields)
+    data = torch.zeros(L, dtype=torch.uint8, device="cuda")
+    batch = DeviceBatch([_device_bytes_column(f.name, data, L) for f in fields], 1)
+    with pytest.raises(ArkError) as e:
+        enc.process_device(batch)
     assert e.value.kind == "Process" and "2 GiB" in e.value.message, e.value.message
