@@ -25,9 +25,31 @@ static std::map<std::string, TimingEntry> g_timing_map;
 
 void note_launch(const char*) { g_launches.fetch_add(1, std::memory_order_relaxed); }
 int64_t launch_count() { return g_launches.load(); }
-void timing_enable(int on) { g_timing.store(on); }
 static void resolve_pending_locked();
-void timing_reset() { std::lock_guard<std::mutex> l(g_timing_mu); resolve_pending_locked(); g_timing_map.clear(); }
+struct PendingTiming { const char* name; const char* also; cudaEvent_t e0, e1; };
+static std::vector<PendingTiming> g_pending;
+static std::vector<cudaEvent_t> g_event_pool;
+// Creating an event costs about as much as two records (measured on H100), so timed launches never create theirs: the
+// pool is stocked when timing is switched on, and each timed launch hands back the events of launches that have ended.
+constexpr size_t EVENT_STOCK = 16;
+void timing_enable(int on) {
+  if (on) {
+    std::lock_guard<std::mutex> l(g_timing_mu);
+    while (g_event_pool.size() < EVENT_STOCK) {
+      cudaEvent_t e = nullptr;
+      if (cudaEventCreate(&e) != cudaSuccess) { cudaGetLastError(); break; }
+      g_event_pool.push_back(e);
+    }
+  }
+  g_timing.store(on);
+}
+static cudaEvent_t g_gap_open = nullptr;  // ARK_TRACE: recorded after the last filter kernel, closed by the next one's start
+void timing_reset() {
+  std::lock_guard<std::mutex> l(g_timing_mu);
+  resolve_pending_locked();
+  g_timing_map.clear();
+  if (g_gap_open) { g_event_pool.push_back(g_gap_open); g_gap_open = nullptr; }  // a gap starts inside the measured window
+}
 bool timing_get(const char* name, double* ms, int64_t* n) {
   std::lock_guard<std::mutex> l(g_timing_mu);
   resolve_pending_locked();
@@ -38,9 +60,6 @@ bool timing_get(const char* name, double* ms, int64_t* n) {
 
 // Timed launches record an event pair and resolve it lazily (no synchronisation on the launch path):
 // ark_kernel_timing_get() is called after the caller has synchronised the device.
-struct PendingTiming { const char* name; const char* also; cudaEvent_t e0, e1; };
-static std::vector<PendingTiming> g_pending;
-static std::vector<cudaEvent_t> g_event_pool;
 
 static cudaEvent_t take_event() {
   {
@@ -52,22 +71,40 @@ static cudaEvent_t take_event() {
   return e;
 }
 
+static void resolve_one_locked(const PendingTiming& p, bool ended) {
+  float ms = 0;
+  if (ended && cudaEventElapsedTime(&ms, p.e0, p.e1) == cudaSuccess) {
+    auto& e = g_timing_map[p.name]; e.ms += ms; e.n += 1;
+    if (p.also) { auto& a = g_timing_map[p.also]; a.ms += ms; a.n += 1; }
+  } else cudaGetLastError();
+  g_event_pool.push_back(p.e0); g_event_pool.push_back(p.e1);
+}
+
 static void resolve_pending_locked() {
-  for (auto& p : g_pending) {
-    float ms = 0;
-    if (cudaEventSynchronize(p.e1) == cudaSuccess && cudaEventElapsedTime(&ms, p.e0, p.e1) == cudaSuccess) {
-      auto& e = g_timing_map[p.name]; e.ms += ms; e.n += 1;
-      if (p.also) { auto& a = g_timing_map[p.also]; a.ms += ms; a.n += 1; }
-    } else cudaGetLastError();
-    g_event_pool.push_back(p.e0); g_event_pool.push_back(p.e1);
-  }
+  for (auto& p : g_pending) resolve_one_locked(p, cudaEventSynchronize(p.e1) == cudaSuccess);
   g_pending.clear();
+}
+
+// The pairs whose launch has ended, without waiting for the others.
+static void resolve_ended_locked() {
+  size_t keep = 0;
+  for (size_t i = 0; i < g_pending.size(); ++i) {
+    const cudaError_t q = cudaEventQuery(g_pending[i].e1);
+    if (q == cudaErrorNotReady) { g_pending[keep++] = g_pending[i]; continue; }
+    resolve_one_locked(g_pending[i], q == cudaSuccess);
+  }
+  g_pending.resize(keep);
+  if (keep && cudaPeekAtLastError() == cudaErrorNotReady) cudaGetLastError();  // "not ready" is an answer, not an error
 }
 
 KernelTimer::KernelTimer(const char* n, cudaStream_t s, const char* a) : name(n), also(a), stream(s) {
   note_launch(n);
   if (g_timing.load(std::memory_order_relaxed)) {
-    e0 = take_event(); e1 = take_event();
+    {
+      std::lock_guard<std::mutex> l(g_timing_mu);  // both events in one visit to the pool
+      if (g_event_pool.size() >= 2) { e0 = g_event_pool.back(); g_event_pool.pop_back(); e1 = g_event_pool.back(); g_event_pool.pop_back(); }
+    }
+    if (!e0) { e0 = take_event(); e1 = take_event(); }
     cudaEventRecord(e0, stream);
   }
 }
@@ -76,7 +113,29 @@ KernelTimer::~KernelTimer() {
     cudaEventRecord(e1, stream);
     std::lock_guard<std::mutex> l(g_timing_mu);
     g_pending.push_back({name, also, e0, e1});
+    resolve_ended_locked();  // the kernel is queued: this host time is not between kernels
   }
+}
+
+bool trace_enabled() { static const bool on = getenv("ARK_TRACE") != nullptr; return on; }
+thread_local CallTrace tl_call_trace;
+
+void trace_kernel_begin(cudaStream_t s) {
+  if (!trace_enabled()) return;
+  cudaEvent_t e = take_event();
+  cudaEventRecord(e, s);
+  std::lock_guard<std::mutex> l(g_timing_mu);
+  if (g_gap_open) g_pending.push_back({"filter_call_gap", nullptr, g_gap_open, e});
+  else g_event_pool.push_back(e);
+  g_gap_open = nullptr;
+}
+void trace_kernel_end(cudaStream_t s) {
+  if (!trace_enabled()) return;
+  cudaEvent_t e = take_event();
+  cudaEventRecord(e, s);
+  std::lock_guard<std::mutex> l(g_timing_mu);
+  if (g_gap_open) g_event_pool.push_back(g_gap_open);
+  g_gap_open = e;
 }
 
 // ---- device binding ---------------------------------------------------------------------------------
@@ -254,21 +313,38 @@ BufferPtr pinned_alloc(size_t bytes) {
 
 // ---- streams ------------------------------------------------------------------------------------------
 static std::mutex g_stream_mu;
-static std::vector<cudaStream_t> g_streams;
+static thread_local std::vector<StreamLease*> tl_leases;  // the leases this thread holds, innermost last
+static std::vector<std::pair<cudaStream_t, FilterScratch*>> g_streams;  // the scratch is never freed, like the stream
 StreamLease::StreamLease() {
   ensure_device();
   {
     std::lock_guard<std::mutex> l(g_stream_mu);
-    if (!g_streams.empty()) { s = g_streams.back(); g_streams.pop_back(); ++tl_lease_depth; return; }
+    if (!g_streams.empty()) {
+      s = g_streams.back().first; filter = g_streams.back().second; g_streams.pop_back();
+      ++tl_lease_depth;
+      tl_leases.push_back(this);
+      return;
+    }
   }
   ARK_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
+  filter = new FilterScratch();
   ++tl_lease_depth;
+  tl_leases.push_back(this);
+}
+FilterScratch* lease_filter_scratch(cudaStream_t s) {
+  for (auto it = tl_leases.rbegin(); it != tl_leases.rend(); ++it) if ((*it)->s == s) return (*it)->filter;
+  return nullptr;
+}
+void StreamLease::synchronize_last() {
+  ARK_CUDA(cudaStreamSynchronize(s));
+  synced = true;
 }
 StreamLease::~StreamLease() {
-  cudaStreamSynchronize(s);  // whatever this call queued is done: its temporaries may now serve any other call
+  if (!synced) cudaStreamSynchronize(s);  // whatever this call queued is done: its temporaries may now serve any other call
+  tl_leases.erase(std::find(tl_leases.begin(), tl_leases.end(), this));
   {
     std::lock_guard<std::mutex> l(g_stream_mu);
-    g_streams.push_back(s);
+    g_streams.push_back({s, filter});
   }
   if (--tl_lease_depth == 0 && !tl_parked.empty()) {
     std::vector<std::pair<BlockPool*, void*>> v;
@@ -554,12 +630,14 @@ __global__ void gather_extents_kernel(const int32_t* const* offs, const int64_t*
 }
 
 Batch import_device(const ArrowDeviceArray* darr, const ArrowSchema* schema, const std::vector<bool>* needed,
-                    BufferPtr keep, bool codec_types) {
+                    BufferPtr keep, bool codec_types, const std::vector<Field>* known_fields) {
   if (darr->device_type != ARROW_DEVICE_CUDA && darr->device_type != ARROW_DEVICE_CUDA_HOST)
     fail(ARK_ERR_PROCESS, "Registration failed: ArrowDeviceArray is not on a CUDA device");
   const ArrowArray* arr = &darr->array;
   if (darr->sync_event) ARK_CUDA(cudaEventSynchronize(*(cudaEvent_t*)darr->sync_event));
-  std::vector<Field> fields = schema_fields(schema);
+  std::vector<Field> parsed;
+  if (!known_fields) parsed = schema_fields(schema);
+  const std::vector<Field>& fields = known_fields ? *known_fields : parsed;
   if (arr->n_children != (int64_t)fields.size())
     fail(ARK_ERR_PROCESS, "Registration failed: array/schema child count mismatch");
   if (arr->offset != 0) fail(ARK_ERR_UNSUPPORTED, "struct array with non-zero offset");
@@ -915,13 +993,15 @@ void export_host(const Batch& b, cudaStream_t stream, ArrowArray* out, ArrowSche
   export_schema(b, out_schema);
 }
 
-void export_device(const Batch& b, ArrowDeviceArray* out, ArrowSchema* out_schema) {
-  StreamLease lease;
+void export_device(const Batch& b, ArrowDeviceArray* out, ArrowSchema* out_schema, StreamLease* caller_lease) {
+  std::unique_ptr<StreamLease> own;
+  if (!caller_lease) own = std::make_unique<StreamLease>();
+  StreamLease& lease = caller_lease ? *caller_lease : *own;
   std::vector<ExportCol> cols;
   for (auto& c : b.cols) cols.push_back(normalise_for_export(c, false, lease.s));
   memset(out, 0, sizeof(*out));
   build_struct_array(b, cols, false, lease.s, &out->array, nullptr);
-  ARK_CUDA(cudaStreamSynchronize(lease.s));
+  lease.synchronize_last();
   int dev = 0; cudaGetDevice(&dev);
   out->device_id = dev; out->device_type = ARROW_DEVICE_CUDA; out->sync_event = nullptr;
   export_schema(b, out_schema);

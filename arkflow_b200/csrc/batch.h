@@ -68,15 +68,31 @@ struct ExportAllocScope {
 };
 
 // ---- streams ------------------------------------------------------------------------------------
+// Scratch of the filter fast path that lives as long as its stream.  Calls on one stream are serialised, so whoever
+// holds the stream's lease owns it outright (engine.cu:try_fast_filter).
+struct FilterScratch {
+  BufferPtr desc[2];                     // look-back descriptors, used by consecutive launches in turn
+  size_t desc_bytes[2] = {0, 0};
+  int64_t zeroed_for[2] = {-1, -1};      // tile count whose descriptor words are known to be zero; -1 = unknown
+  int next = 0;                          // the buffer the next launch uses
+  BufferPtr totals;                      // pinned: the last tile's row and byte totals
+};
+
 // RAII lease of a non-blocking stream from a small pool (replaces the reference's
 // SessionContextPool::acquire/release, context_pool.rs:91-119, without its leak-on-error).
 struct StreamLease {
   StreamLease();
   ~StreamLease();
+  // Synchronises the stream.  The caller promises to queue nothing more on it, so the lease ends without a second one.
+  void synchronize_last();
   cudaStream_t s;
+  FilterScratch* filter;
+  bool synced = false;
   StreamLease(const StreamLease&) = delete;
   StreamLease& operator=(const StreamLease&) = delete;
 };
+// The filter scratch of the stream `s` when the calling thread holds its lease, else nullptr.
+FilterScratch* lease_filter_scratch(cudaStream_t s);
 
 // ---- columns and batches ------------------------------------------------------------------------
 struct Field {
@@ -142,8 +158,9 @@ inline int fixed_width(DType t) {
 // columns (formats i, I, L, f): only arrow_to_protobuf reads them; every other caller leaves them not present.
 Batch import_host(const ArrowArray* arr, const ArrowSchema* schema, const std::vector<bool>* needed,
                   cudaStream_t stream, int64_t* h2d_bytes = nullptr, bool codec_types = false);
+// `fields`: schema_fields(schema) when the caller has it already.
 Batch import_device(const ArrowDeviceArray* arr, const ArrowSchema* schema, const std::vector<bool>* needed,
-                    BufferPtr keep, bool codec_types = false);
+                    BufferPtr keep, bool codec_types = false, const std::vector<Field>* fields = nullptr);
 
 // Export: builds a struct ArrowArray/ArrowSchema whose release callbacks drop the owners.
 // Host export copies HBM → pinned host on `stream` and synchronizes it.
@@ -151,7 +168,9 @@ void export_schema(const Batch& b, ArrowSchema* out);
 void export_empty_schema(ArrowSchema* out);  // RecordBatch::new_empty(Schema::empty()), sql.rs:137-139
 void export_host(const Batch& b, cudaStream_t stream, ArrowArray* out, ArrowSchema* out_schema,
                  int64_t* d2h_bytes = nullptr);
-void export_device(const Batch& b, ArrowDeviceArray* out, ArrowSchema* out_schema);
+// Device export queues its few normalising kernels on `lease`'s stream (a lease of its own when null) and ends with that
+// stream's last synchronize.
+void export_device(const Batch& b, ArrowDeviceArray* out, ArrowSchema* out_schema, StreamLease* lease = nullptr);
 
 // Moves an ArrowArray into shared ownership: the returned pointer releases it when dropped.
 BufferPtr adopt_array(ArrowArray* arr);

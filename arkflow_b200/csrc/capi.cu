@@ -37,13 +37,6 @@ SqlProcessor* as_sql(ark_proc_t* p) {
   return static_cast<SqlProcessor*>(p->impl.get());
 }
 
-std::vector<bool> needed_mask(const Plan& plan, size_t n_fields) {
-  std::vector<bool> m(n_fields, false);
-  if (plan.identity) { std::fill(m.begin(), m.end(), true); return m; }
-  for (int c : plan.used_cols) m[c] = true;
-  return m;
-}
-
 void set_none(ArrowArray* out, ArrowSchema* out_schema) {
   memset(out, 0, sizeof(*out));
   if (out_schema) memset(out_schema, 0, sizeof(*out_schema));
@@ -111,27 +104,34 @@ int ark_sql_process_device(ark_proc_t* p, ArrowDeviceArray* in, ArrowSchema* in_
     ArrowDeviceArray view = *in;
     view.array = *(const ArrowArray*)in_owner.get();
     if (view.array.length == 0) { memset(out, 0, sizeof(*out)); if (out_schema) memset(out_schema, 0, sizeof(*out_schema)); return; }
-    static const bool trace = getenv("ARK_TRACE") != nullptr;  // per-phase host time of this entry point, to stderr
+    const bool trace = trace_enabled();  // per-phase host time of this entry point, to stderr
     auto now = [] { return std::chrono::steady_clock::now(); };
     auto us = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) {
       return (double)std::chrono::duration_cast<std::chrono::nanoseconds>(b - a).count() / 1e3;
     };
     const auto t0 = now();
-    std::vector<Field> fields = schema_fields(in_schema);
-    auto plan = sp->plan_for(fields);
-    std::vector<bool> mask = needed_mask(*plan, fields.size());
+    tl_call_trace = CallTrace{t0, t0, t0};  // stays at t0 unless the filter fast path ran
+    auto bound = sp->bind(in_schema);
     const auto t1 = now();
     StreamLease lease;
-    Batch b = import_device(&view, in_schema, &mask, in_owner);
+    Batch b = import_device(&view, in_schema, &bound->mask, in_owner, false, &bound->fields);
     const auto t2 = now();
-    Batch r = sp->execute(*plan, b, lease.s);
+    Batch r = sp->execute(*bound->plan, b, lease.s);
     const auto t3 = now();
-    ARK_CUDA(cudaStreamSynchronize(lease.s));
-    export_device(r, out, out_schema);
+    export_device(r, out, out_schema, &lease);
+    const auto t4 = now();
+    // the input's release (an outside callback) runs here, unless an exported column still aliases it
+    r = Batch();
+    b = Batch();
+    in_owner.reset();
     if (trace) {
-      const auto t4 = now();
-      fprintf(stderr, "[ark trace] sql_process_device: plan %.1f us, import %.1f us, execute %.1f us, export %.1f us\n", us(t0, t1), us(t1, t2),
-              us(t2, t3), us(t3, t4));
+      const auto t5 = now();
+      const CallTrace& ct = tl_call_trace;
+      fprintf(stderr,
+              "[ark trace] sql_process_device: plan %.1f us, import %.1f us, execute %.1f us (to launch enqueued %.1f us = outputs and "
+              "scratch %.1f us + launch %.1f us, gpu wait %.1f us), sync return to export done %.1f us, input release %.1f us, total %.1f us\n",
+              us(t0, t1), us(t1, t2), us(t2, t3), us(t2, ct.launched), us(t2, ct.prepared), us(ct.prepared, ct.launched),
+              us(ct.launched, ct.synced), us(ct.synced, t4), us(t4, t5), us(t0, t5));
     }
   });
 }

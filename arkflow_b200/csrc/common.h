@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <chrono>
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
@@ -43,6 +44,16 @@ struct KernelTimer {  // RAII: records CUDA events around one launch when timing
   cudaStream_t stream;
   cudaEvent_t e0 = nullptr, e1 = nullptr;
 };
+
+// ---- ARK_TRACE (opt-in, off by default) ----
+// Host timestamps of one filter fast-path call (ark_sql_process_device prints its phases from them), and the GPU idle time
+// between consecutive filter kernels: an event after one kernel and an event before the next, resolved lazily like the
+// kernel timers and read as ark_kernel_timing_get("filter_call_gap").
+bool trace_enabled();
+void trace_kernel_begin(cudaStream_t s);
+void trace_kernel_end(cudaStream_t s);
+struct CallTrace { std::chrono::steady_clock::time_point prepared, launched, synced; };
+extern thread_local CallTrace tl_call_trace;
 
 void bind_device(int device);   // remembered by ark_b200_init
 void ensure_device();           // re-binds the calling host thread to that device

@@ -51,6 +51,41 @@ std::shared_ptr<const Plan> SqlProcessor::plan_for(const std::vector<Field>& fie
   return plan;
 }
 
+std::vector<bool> needed_mask(const Plan& plan, size_t n_fields) {
+  std::vector<bool> m(n_fields, false);
+  if (plan.identity) { std::fill(m.begin(), m.end(), true); return m; }
+  for (int c : plan.used_cols) m[c] = true;
+  return m;
+}
+
+static bool same_schema(const ArrowSchema* s, const std::vector<Field>& f) {
+  if (!s || !s->format || strcmp(s->format, "+s") != 0 || s->n_children != (int64_t)f.size()) return false;
+  for (size_t i = 0; i < f.size(); ++i) {
+    const ArrowSchema* c = s->children[i];
+    if (strcmp(c->name ? c->name : "", f[i].name.c_str()) != 0 || strcmp(c->format ? c->format : "", f[i].format.c_str()) != 0 ||
+        ((c->flags & ARROW_FLAG_NULLABLE) != 0) != f[i].nullable)
+      return false;
+  }
+  return true;
+}
+
+std::shared_ptr<const SqlProcessor::BoundSchema> SqlProcessor::bind(const ArrowSchema* schema) {
+  {
+    std::lock_guard<std::mutex> l(mu_);
+    if (last_bound_ && same_schema(schema, last_bound_->fields)) {
+      if (last_bound_->plan->kind == Plan::Aggregate) last_agg_ = last_bound_->plan;  // as plan_for does
+      return last_bound_;
+    }
+  }
+  auto b = std::make_shared<BoundSchema>();
+  b->fields = schema_fields(schema);
+  b->plan = plan_for(b->fields);
+  b->mask = needed_mask(*b->plan, b->fields.size());
+  std::lock_guard<std::mutex> l(mu_);
+  last_bound_ = b;
+  return b;
+}
+
 std::shared_ptr<const Plan> SqlProcessor::last_aggregate_plan() {
   std::lock_guard<std::mutex> l(mu_);
   return last_agg_;
@@ -113,7 +148,8 @@ size_t filter_project_tma_desc_words(int64_t n_tiles);
 void filter_project_tma_note_avg_len(double avg);
 bool launch_filter_project_tma(int64_t n_rows, const void* pred_in, int n_fixed_out, const void* const* fixed_in, void* const* fixed_out,
                                const int32_t* offsets_in, const uint8_t* data_in, int64_t data_bytes, int32_t* offsets_out, uint8_t* data_out,
-                               int cmp, int is_f64, uint64_t constant, unsigned long long* desc, long long* totals, cudaStream_t stream);
+                               int cmp, int is_f64, uint64_t constant, unsigned long long* desc, unsigned long long* desc_next,
+                               long long* totals, cudaStream_t stream);
 
 // SELECT <fixed-width cols…> [, <1 var-len col>] WHERE <fixed col> <cmp> <literal>, no NULLs in the used columns.
 static bool try_fast_filter(const Plan& plan, Batch& in, Batch& out, cudaStream_t stream) {
@@ -137,28 +173,53 @@ static bool try_fast_filter(const Plan& plan, Batch& in, Batch& out, cudaStream_
   void* fout[8] = {nullptr};
   std::vector<BufferPtr> fbuf(fixed_outs.size());
   BufferPtr obuf, dbuf;
-  for (size_t c = 0; c < fixed_outs.size(); ++c) {
-    fin[c] = src_col(plan.outputs[fixed_outs[c]].src.slot).data;
-    fbuf[c] = device_alloc((size_t)n * 8 + 16);
-    fout[c] = fbuf[c].get();
-  }
   const Column* vs = varlen_out >= 0 ? &src_col(plan.outputs[varlen_out].src.slot) : nullptr;
-  if (vs) { obuf = device_alloc((size_t)(n + 1) * 4 + 16); dbuf = device_alloc((size_t)std::max<int64_t>(varlen_bytes_bound(*vs), 0) + 32); }
+  {  // every output buffer is cut from one pool block (one allocation and one free per call); each piece is 256-byte aligned
+    auto piece = [](size_t bytes) { return (size_t)round_up((int64_t)bytes, 256); };
+    const size_t fixed_bytes = piece((size_t)n * 8 + 16), off_bytes = vs ? piece((size_t)(n + 1) * 4 + 16) : 0;
+    const size_t data_bytes = vs ? piece((size_t)std::max<int64_t>(varlen_bytes_bound(*vs), 0) + 32) : 0;
+    BufferPtr block = device_alloc(fixed_bytes * fixed_outs.size() + off_bytes + data_bytes);
+    uint8_t* p = (uint8_t*)block.get();
+    for (size_t c = 0; c < fixed_outs.size(); ++c, p += fixed_bytes) {
+      fin[c] = src_col(plan.outputs[fixed_outs[c]].src.slot).data;
+      fbuf[c] = BufferPtr(block, p);
+      fout[c] = p;
+    }
+    if (vs) { obuf = BufferPtr(block, p); dbuf = BufferPtr(block, p + off_bytes); }
+  }
+  // Look-back descriptors: the stream's two buffers in turn.  Each launch's tiles zero, in the other buffer, the words the
+  // next launch with the same tile count reads; calls on one stream are serialised, so nothing reads that buffer meanwhile.
+  // A buffer whose state is unknown or that was zeroed for another tile count is cleared with one memset.
+  FilterScratch unleased;  // a stream this thread does not lease: nothing is known about its buffers
+  FilterScratch* leased = lease_filter_scratch(stream);
+  FilterScratch& fs = leased ? *leased : unleased;
   const size_t desc_bytes = filter_project_tma_desc_words(n_tiles) * 8;
-  BufferPtr desc = device_alloc(desc_bytes);
-  ARK_CUDA(cudaMemsetAsync(desc.get(), 0, desc_bytes, stream));
+  const int cur = fs.next, other = cur ^ 1;
+  for (int k : {cur, other})
+    if (fs.desc_bytes[k] < desc_bytes) {
+      fs.desc[k] = device_alloc(desc_bytes);
+      fs.desc_bytes[k] = desc_bytes;
+      fs.zeroed_for[k] = -1;
+    }
+  if (fs.zeroed_for[cur] != n_tiles) ARK_CUDA(cudaMemsetAsync(fs.desc[cur].get(), 0, desc_bytes, stream));
   // the kernel's last tile stores the two totals straight into pinned host memory (device-accessible under unified
   // addressing): one stream synchronize, no separate device→host copy on the critical path of every call
-  BufferPtr host_res = pinned_alloc(64);
-  long long* totals = (long long*)host_res.get();
+  if (!fs.totals) fs.totals = pinned_alloc(64);
+  long long* totals = (long long*)fs.totals.get();
+  fs.zeroed_for[cur] = -1;
+  if (trace_enabled()) tl_call_trace.prepared = std::chrono::steady_clock::now();
   if (!launch_filter_project_tma(n, src_col(plan.simple.slot).data, (int)fixed_outs.size(), fin, fout, vs ? vs->offsets : nullptr,
                                  vs ? vs->data : nullptr, vs ? vs->data_bytes : 0 /* -1 = unknown */, vs ? (int32_t*)obuf.get() : nullptr,
                                  vs ? (uint8_t*)dbuf.get() : nullptr, plan.simple.cmp, plan.simple.is_f64, plan.simple.constant,
-                                 (unsigned long long*)desc.get(), totals, stream))
+                                 (unsigned long long*)fs.desc[cur].get(), (unsigned long long*)fs.desc[other].get(), totals, stream))
     return false;
   ARK_CUDA(cudaGetLastError());
+  fs.zeroed_for[other] = n_tiles;
+  fs.next = other;
+  if (trace_enabled()) tl_call_trace.launched = std::chrono::steady_clock::now();
   ARK_CUDA(cudaStreamSynchronize(stream));
-  const int64_t count = ((const int64_t*)host_res.get())[0], bytes = ((const int64_t*)host_res.get())[1];
+  if (trace_enabled()) tl_call_trace.synced = std::chrono::steady_clock::now();
+  const int64_t count = totals[0], bytes = totals[1];
   if (vs && count > 0) filter_project_tma_note_avg_len((double)bytes / (double)count);
   out.cols.resize(plan.outputs.size());
   out.num_rows = count;

@@ -54,6 +54,12 @@ struct SqlProcessor : Processor {
   std::shared_ptr<const Plan> join_plan_for(const std::vector<std::string>& names,
                                             const std::vector<std::vector<Field>>& tables);
 
+  // An input schema bound to this processor's query: its fields, the plan and which columns the plan reads.  The most
+  // recent one is kept, and a schema that matches it field for field (a stream of batches of one schema) is bound again
+  // without parsing it, fingerprinting it or looking the plan up.
+  struct BoundSchema { std::vector<Field> fields; std::shared_ptr<const Plan> plan; std::vector<bool> mask; };
+  std::shared_ptr<const BoundSchema> bind(const ArrowSchema* schema);
+
   // Runs the bound plan on an HBM-resident batch.  `in` must contain the plan's used columns.
   Batch execute(const Plan& plan, Batch& in, cudaStream_t stream);
 
@@ -61,7 +67,11 @@ struct SqlProcessor : Processor {
   std::mutex mu_;
   std::map<std::string, std::shared_ptr<const Plan>> plans_;
   std::shared_ptr<const Plan> last_agg_;
+  std::shared_ptr<const BoundSchema> last_bound_;
 };
+
+// Which of `n_fields` input columns the plan reads (all of them for SELECT *).
+std::vector<bool> needed_mask(const Plan& plan, size_t n_fields);
 
 Batch run_filter_project(const Plan& plan, Batch& in, cudaStream_t stream);
 Batch run_aggregate(const Plan& plan, Batch& in, cudaStream_t stream);

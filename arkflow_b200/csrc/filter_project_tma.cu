@@ -50,6 +50,7 @@ struct TmaParams {
   int32_t* offsets_out;
   uint8_t* data_out;
   unsigned long long* desc;
+  unsigned long long* desc_next;            // or null: its tile (and group) descriptor words are zeroed for the next launch
   long long* totals;
   int32_t debug;                            // measurement knob (ARK_FP_DEBUG): bit 0 = skip the look-back (results are garbage), bit 2 = force helping
   int32_t lb_delay;                         // ns the look-back warp sleeps before its first poll
@@ -312,6 +313,10 @@ __global__ void __launch_bounds__(DT + 32) __maxnreg__(MAXR) filter_project_tile
     else lookback_two_level<VARLEN>(P, tile, tile_cnt, tb, lane, &ex0, &ex1);
     if (lane == 0) { s_excl[0] = ex0; s_excl[1] = ex1; }
     __syncthreads();   // (2)
+    if (P.desc_next && lane == 0) {  // no launch reads desc_next before this one has ended
+      P.desc_next[(size_t)tile * DESC_STRIDE] = 0;
+      if ((tile & 31) == 0) P.desc_next[((size_t)n_tiles + (tile >> 5)) * DESC_STRIDE] = 0;
+    }
     return;
   }
   const int64_t row0 = (int64_t)tile * TT;
@@ -469,10 +474,12 @@ size_t filter_project_tma_desc_words(int64_t n_tiles) { return (size_t)(n_tiles 
 int filter_project_tma_max_fixed_out() { return T_MAX_FIXED_OUT; }
 
 // Returns false when the inputs do not meet the alignment rules of this path, or when the query projects no column this
-// kernel writes (caller falls back).  `desc` holds filter_project_tma_desc_words(tiles) zeroed words.
+// kernel writes (caller falls back).  `desc` holds filter_project_tma_desc_words(tiles) zeroed words.  `desc_next` (may be
+// null) is another buffer of that size: the kernel zeroes in it the descriptor words a launch with the same tile count reads.
 bool launch_filter_project_tma(int64_t n_rows, const void* pred_in, int n_fixed_out, const void* const* fixed_in, void* const* fixed_out,
                                const int32_t* offsets_in, const uint8_t* data_in, int64_t data_bytes, int32_t* offsets_out, uint8_t* data_out,
-                               int cmp, int is_f64, uint64_t constant, unsigned long long* desc, long long* totals, cudaStream_t stream) {
+                               int cmp, int is_f64, uint64_t constant, unsigned long long* desc, unsigned long long* desc_next,
+                               long long* totals, cudaStream_t stream) {
   if (reinterpret_cast<uintptr_t>(pred_in) & 7) return false;
   if (n_rows >= (1ll << 31) - 1) return false;  // 31-bit descriptor fields
   if (data_out && (reinterpret_cast<uintptr_t>(data_out) & 15)) return false;
@@ -502,7 +509,7 @@ bool launch_filter_project_tma(int64_t n_rows, const void* pred_in, int n_fixed_
     if (fixed_in[c] == pred_in) P.fixed_is_pred |= 1u << c;
   }
   P.offsets_in = offsets_in; P.data_in = data_in; P.offsets_out = offsets_out; P.data_out = data_out;
-  P.desc = desc; P.totals = totals;
+  P.desc = desc; P.desc_next = desc_next; P.totals = totals;
   static const int debug = [] { const char* e = getenv("ARK_FP_DEBUG"); return e ? atoi(e) : 0; }();
   P.debug = debug;
   // the look-back warp sleeps this long before its first poll: the aggregates it needs belong to tiles whose loads were issued
@@ -537,7 +544,9 @@ bool launch_filter_project_tma(int64_t n_rows, const void* pred_in, int n_fixed_
   else return false;  // before the timer: a declined launch is not recorded
   KernelTimer t("filter_project_tma_kernel", stream, "filter_project_tile_kernel");
   void* args[] = {(void*)&P};
+  trace_kernel_begin(stream);
   ARK_CUDA(cudaLaunchKernel(fn, dim3(P.n_tiles), dim3(T_THREADS + 32), args, smem, stream));
+  trace_kernel_end(stream);
   return true;
 }
 
