@@ -353,6 +353,8 @@ class DeviceBatch:
                 offsets = up(bufs[1], np.int32, off + n + 1)
                 data = up(bufs[2], np.uint8) if bufs[2] is not None else torch.empty(0, dtype=torch.uint8, device=device)
                 cols.append(DeviceColumn(name, dt, n, data, offsets, validity, arr.null_count, f.nullable, off))
+            elif pa.types.is_null(arr.type):
+                cols.append(DeviceColumn(name, "null", n, None, None, None, n, f.nullable))
             else:
                 raise TypeError(f"unsupported Arrow type for device upload: {arr.type}")
         return DeviceBatch(cols, rb.num_rows)

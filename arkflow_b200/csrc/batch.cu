@@ -893,7 +893,9 @@ static ExportCol normalise_for_export(const Column& c_in, bool to_host, cudaStre
     case DType::Utf8: case DType::Binary: {
       e.n_buffers = 3;
       e.buf1_bytes = (n + 1) * 4;
-      if (!to_host) {  // device export: Arrow does not require offsets[0] == 0; hand the buffers over as they are
+      // device export: Arrow does not require offsets[0] == 0; hand the buffers over as they are, unless offsets[0] != 0 is
+      // known.  A host import points `data` offsets[0] bytes before its allocation, which no consumer may be handed.
+      if (!to_host && c.first_offset == 0) {
         if (c.offsets) e.buf1 = c.offsets;
         else { BufferPtr o = device_alloc(4); ARK_CUDA(cudaMemsetAsync(o.get(), 0, 4, stream)); e.buf1 = o.get(); e.owners.push_back(o); }
         e.buf2 = c.data; e.buf2_bytes = std::max<int64_t>(c.data_bytes, 0);

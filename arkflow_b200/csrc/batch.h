@@ -155,7 +155,8 @@ inline int fixed_width(DType t) {
 // `stream` (the source is read asynchronously when pinned; the caller synchronizes before
 // releasing `arr`).  Device import wraps the pointers without copying; `keep` (may be null) is
 // attached to every column as an owner.  `codec_types` also imports Int32 / UInt32 / UInt64 / Float32
-// columns (formats i, I, L, f): only arrow_to_protobuf reads them; every other caller leaves them not present.
+// columns (formats i, I, L, f): arrow_to_protobuf reads them and concat carries them (concat_batches, the buffers, `batch`);
+// every other caller leaves them not present.
 Batch import_host(const ArrowArray* arr, const ArrowSchema* schema, const std::vector<bool>* needed,
                   cudaStream_t stream, int64_t* h2d_bytes = nullptr, bool codec_types = false);
 // `fields`: schema_fields(schema) when the caller has it already.

@@ -296,7 +296,7 @@ int ark_buffer_write(ark_buf_t* b, ArrowArray* in, ArrowSchema* in_schema, const
     const ArrowArray* arr = (const ArrowArray*)in_owner.get();
     if (!arr) fail(ARK_ERR_PROCESS, "input array already released");
     StreamLease lease;
-    Batch batch = import_host(arr, in_schema, nullptr, lease.s);  // the window lives in HBM from here on
+    Batch batch = import_host(arr, in_schema, nullptr, lease.s, nullptr, true);  // the window lives in HBM from here on
     ARK_CUDA(cudaStreamSynchronize(lease.s));
     buffer_enqueue(b, std::move(batch), input_name, ack_token);
   });
@@ -311,7 +311,7 @@ int ark_buffer_write_device(ark_buf_t* b, ArrowDeviceArray* in, ArrowSchema* in_
     if (!in_owner) fail(ARK_ERR_PROCESS, "input array already released");
     ArrowDeviceArray view = *in;
     view.array = *(const ArrowArray*)in_owner.get();
-    Batch batch = import_device(&view, in_schema, nullptr, in_owner);
+    Batch batch = import_device(&view, in_schema, nullptr, in_owner, true);
     buffer_enqueue(b, std::move(batch), input_name, ack_token);
   });
 }
@@ -470,7 +470,7 @@ int ark_batch_process(ark_batcher_t* b, ArrowArray* in, ArrowSchema* in_schema, 
     Batch batch;
     {
       StreamLease lease;
-      batch = import_host(arr, in_schema, nullptr, lease.s);
+      batch = import_host(arr, in_schema, nullptr, lease.s, nullptr, true);
       ARK_CUDA(cudaStreamSynchronize(lease.s));
     }
     std::lock_guard<std::mutex> l(b->mu);

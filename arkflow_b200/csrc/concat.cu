@@ -99,7 +99,8 @@ struct BitSeg {
   int bit0;
 };
 
-__global__ void concat_bits_kernel(const BitSeg* segs, int n_segs, long long total_rows, uint8_t* out) {
+// `zeros` (may be null): incremented by the number of clear bits gathered, i.e. the NULLs of a validity bitmap
+__global__ void concat_bits_kernel(const BitSeg* segs, int n_segs, long long total_rows, uint8_t* out, unsigned long long* zeros) {
   const long long ob = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (ob >= (total_rows + 7) / 8) return;
   unsigned v = 0;
@@ -109,8 +110,8 @@ __global__ void concat_bits_kernel(const BitSeg* segs, int n_segs, long long tot
     const int mid = (lo + hi + 1) >> 1;
     if (segs[mid].row0 <= r) lo = mid; else hi = mid - 1;
   }
-  int seg = lo;
-  for (int i = 0; i < 8 && r < total_rows; ++i, ++r) {
+  int seg = lo, i = 0;
+  for (; i < 8 && r < total_rows; ++i, ++r) {
     while (seg + 1 < n_segs && segs[seg + 1].row0 <= r) ++seg;
     const BitSeg s = segs[seg];
     const long long p = r - s.row0 + s.bit0;
@@ -118,6 +119,7 @@ __global__ void concat_bits_kernel(const BitSeg* segs, int n_segs, long long tot
     v |= bit << i;
   }
   out[ob] = (uint8_t)v;
+  if (zeros && i != __popc(v)) atomicAdd(zeros, (unsigned long long)(i - __popc(v)));
 }
 
 }  // namespace
@@ -135,12 +137,39 @@ Batch concat_device(std::vector<Batch>& ins, cudaStream_t stream) {
                                   dtype_name(ins[b].cols[c].field.type) + " at column index " + std::to_string(c));
     }
   }
+  // A Null column is a length without buffers: the import marks it not present, as it does every type it holds no
+  // buffers for, so it is told apart by its format.
+  auto null_column = [](const Column& c) { return c.field.type == DType::Null && (c.present || c.field.format == "n"); };
+  for (size_t c = 0; c < ncol; ++c) {
+    const Column& c0 = ins[0].cols[c];
+    const DType t = c0.field.type;
+    if (null_column(c0)) continue;
+    if (!c0.present || (!fixed_width(t) && t != DType::Bool && t != DType::Utf8 && t != DType::Binary))
+      fail(ARK_ERR_UNSUPPORTED, "concat of a column with Arrow type '" + (c0.field.format.empty() ? std::string(dtype_arrow_format(t)) : c0.field.format) + "'");
+  }
+  // RecordBatch::try_new: a field the schema batch declares non-nullable may hold no NULL.  A known null count settles
+  // it here; members whose count is unknown (-1) are counted by concat_bits_kernel, which the one-batch return skips.
+  std::vector<char> count_nulls(ncol, 0);
+  bool any_count = false;
+  auto non_nullable = [&](size_t c) {
+    fail(ARK_ERR_PROCESS, "Merge batches failed: Invalid argument error: Column '" + ins[0].cols[c].field.name +
+                              "' is declared as non-nullable but contains null values");
+  };
+  for (size_t c = 0; c < ncol; ++c) {
+    if (ins[0].cols[c].field.nullable) continue;
+    for (auto& b : ins) {
+      const Column& m = b.cols[c];
+      if (!m.validity || b.num_rows == 0) continue;
+      if (m.null_count > 0) non_nullable(c);
+      if (m.null_count < 0) count_nulls[c] = any_count = true;
+    }
+  }
   {
     std::vector<Column*> all;  // one round trip for the extents of every batch
     for (auto& b : ins) for (auto& c : b.cols) all.push_back(&c);
     resolve_varlen_extents_many(all, stream);
   }
-  if (ins.size() == 1) return ins[0];
+  if (ins.size() == 1 && !any_count) return ins[0];
   int64_t total_rows = 0;
   std::vector<int64_t> row0(ins.size());
   for (size_t b = 0; b < ins.size(); ++b) { row0[b] = total_rows; total_rows += ins[b].num_rows; }
@@ -151,29 +180,32 @@ Batch concat_device(std::vector<Batch>& ins, cudaStream_t stream) {
   std::vector<CopySpan> spans;
   std::vector<BufferPtr> keep;
   struct PendingOffsets { std::vector<OffsetSeg> segs; int32_t* out; int64_t total_bytes; };
-  struct PendingBits { std::vector<BitSeg> segs; uint8_t* out; };
+  struct PendingBits { std::vector<BitSeg> segs; uint8_t* out; int counter; };  // counter: slot in `zeros`, or -1
   std::vector<PendingOffsets> poffs;
   std::vector<PendingBits> pbits;
+  std::vector<size_t> counted;  // column of each `zeros` slot
   auto add_span = [&](const uint8_t* src, uint8_t* dst, int64_t bytes) {
     if (bytes > 0) spans.push_back({src, dst, (unsigned long long)bytes, 0});
   };
   for (size_t c = 0; c < ncol; ++c) {
     const Column& c0 = ins[0].cols[c];
-    if (!c0.present) fail(ARK_ERR_UNSUPPORTED, "concat of a column with Arrow type '" + c0.field.format + "'");
     Column oc;
     oc.field = c0.field; oc.length = total_rows;
+    if (null_column(c0)) { out.cols.push_back(std::move(oc)); continue; }
     bool any_null = false;
     for (auto& b : ins) any_null = any_null || (b.cols[c].validity != nullptr);
     switch (c0.field.type) {
-      case DType::Int64: case DType::Float64: {
-        BufferPtr d = device_alloc((size_t)total_rows * 8 + 16);
-        for (size_t b = 0; b < ins.size(); ++b) add_span(ins[b].cols[c].data, (uint8_t*)d.get() + row0[b] * 8, ins[b].num_rows * 8);
-        oc.data = (const uint8_t*)d.get(); oc.data_bytes = total_rows * 8; oc.owners.push_back(d);
+      case DType::Int64: case DType::Float64:
+      case DType::Int32: case DType::UInt32: case DType::UInt64: case DType::Float32: {
+        const int w = fixed_width(c0.field.type);
+        BufferPtr d = device_alloc((size_t)total_rows * w + 16);
+        for (size_t b = 0; b < ins.size(); ++b) add_span(ins[b].cols[c].data, (uint8_t*)d.get() + row0[b] * w, ins[b].num_rows * w);
+        oc.data = (const uint8_t*)d.get(); oc.data_bytes = total_rows * w; oc.owners.push_back(d);
         break;
       }
       case DType::Bool: {
         BufferPtr d = device_alloc((size_t)(total_rows + 7) / 8 + 16);
-        PendingBits pb; pb.out = (uint8_t*)d.get();
+        PendingBits pb; pb.out = (uint8_t*)d.get(); pb.counter = -1;
         for (size_t b = 0; b < ins.size(); ++b) if (ins[b].num_rows) pb.segs.push_back({ins[b].cols[c].data, row0[b], ins[b].cols[c].data_bit0});
         pbits.push_back(std::move(pb));
         oc.data = (const uint8_t*)d.get(); oc.data_bit0 = 0; oc.data_bytes = (total_rows + 7) / 8; oc.owners.push_back(d);
@@ -199,12 +231,13 @@ Batch concat_device(std::vector<Batch>& ins, cudaStream_t stream) {
         oc.owners = {o, d};
         break;
       }
-      default: break;  // Null type: nothing to copy
+      default: break;  // not reached: the types checked above
     }
     if (any_null && total_rows > 0) {
       BufferPtr v = device_alloc((size_t)(total_rows + 7) / 8 + 16);
-      PendingBits pb; pb.out = (uint8_t*)v.get();
+      PendingBits pb; pb.out = (uint8_t*)v.get(); pb.counter = -1;
       for (size_t b = 0; b < ins.size(); ++b) if (ins[b].num_rows) pb.segs.push_back({ins[b].cols[c].validity, row0[b], ins[b].cols[c].validity_bit0});
+      if (count_nulls[c]) { pb.counter = (int)counted.size(); counted.push_back(c); }
       pbits.push_back(std::move(pb));
       oc.validity = (const uint8_t*)v.get(); oc.validity_bit0 = 0; oc.null_count = -1; oc.owners.push_back(v);
     }
@@ -216,6 +249,7 @@ Batch concat_device(std::vector<Batch>& ins, cudaStream_t stream) {
   size_t desc_bytes = spans.size() * sizeof(CopySpan);
   for (auto& p : poffs) desc_bytes += p.segs.size() * sizeof(OffsetSeg);
   for (auto& p : pbits) desc_bytes += p.segs.size() * sizeof(BitSeg);
+  desc_bytes += counted.size() * sizeof(unsigned long long);
   BufferPtr hdesc = pinned_alloc(desc_bytes + 64), ddesc = device_alloc(desc_bytes + 64);
   size_t pos = 0;
   auto put = [&](const void* src, size_t n) -> const void* {
@@ -224,6 +258,10 @@ Batch concat_device(std::vector<Batch>& ins, cudaStream_t stream) {
     pos += n;
     return dptr;
   };
+  // the NULL counters go first: 8-byte aligned, and uploaded as zeros with the descriptors
+  const std::vector<unsigned long long> zero_counts(counted.size(), 0);
+  unsigned long long* d_zeros = (unsigned long long*)put(zero_counts.data(), zero_counts.size() * sizeof(unsigned long long));
+  const unsigned long long* h_zeros = (const unsigned long long*)hdesc.get();
   const CopySpan* d_spans = (const CopySpan*)put(spans.data(), spans.size() * sizeof(CopySpan));
   std::vector<const OffsetSeg*> d_offs;
   std::vector<const BitSeg*> d_bits;
@@ -236,18 +274,25 @@ Batch concat_device(std::vector<Batch>& ins, cudaStream_t stream) {
     concat_copy_kernel<<<grid, CONCAT_THREADS, 0, stream>>>(d_spans, (int)spans.size(), n_chunks);
   }
   for (size_t i = 0; i < poffs.size(); ++i) {
-    KernelTimer t("concat_offsets_kernel", stream);
     if (poffs[i].segs.empty()) { ARK_CUDA(cudaMemsetAsync(poffs[i].out, 0, 4, stream)); continue; }
+    KernelTimer t("concat_offsets_kernel", stream);
     concat_offsets_kernel<<<(unsigned)ceil_div(total_rows + 1, 256), 256, 0, stream>>>(d_offs[i], (int)poffs[i].segs.size(), total_rows,
                                                                                        poffs[i].total_bytes, poffs[i].out);
   }
   for (size_t i = 0; i < pbits.size(); ++i) {
     if (pbits[i].segs.empty()) continue;
     KernelTimer t("concat_bits_kernel", stream);
-    concat_bits_kernel<<<(unsigned)ceil_div((total_rows + 7) / 8, 256), 256, 0, stream>>>(d_bits[i], (int)pbits[i].segs.size(), total_rows, pbits[i].out);
+    concat_bits_kernel<<<(unsigned)ceil_div((total_rows + 7) / 8, 256), 256, 0, stream>>>(d_bits[i], (int)pbits[i].segs.size(), total_rows, pbits[i].out,
+                                                                                       pbits[i].counter < 0 ? nullptr : d_zeros + pbits[i].counter);
   }
   ARK_CUDA(cudaGetLastError());
+  if (!counted.empty())
+    ARK_CUDA(cudaMemcpyAsync((void*)h_zeros, d_zeros, counted.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream));
   ARK_CUDA(cudaStreamSynchronize(stream));  // descriptors live in pooled blocks: finish before they are recycled
+  for (size_t k = 0; k < counted.size(); ++k) {
+    if (h_zeros[k]) non_nullable(counted[k]);
+    out.cols[counted[k]].null_count = 0;
+  }
   return out;
 }
 
@@ -262,7 +307,7 @@ extern "C" int ark_concat_batches(int n, ArrowArray* ins, ArrowSchema* in_schema
     if (n <= 0) fail(ARK_ERR_PROCESS, "Merge batches failed: no batches");
     StreamLease lease;
     std::vector<Batch> bs;
-    for (int i = 0; i < n; ++i) bs.push_back(import_host((const ArrowArray*)owners[i].get(), &in_schemas[i], nullptr, lease.s));
+    for (int i = 0; i < n; ++i) bs.push_back(import_host((const ArrowArray*)owners[i].get(), &in_schemas[i], nullptr, lease.s, nullptr, true));
     Batch r = concat_device(bs, lease.s);
     export_host(r, lease.s, out, out_schema);
     return ARK_OK;
@@ -282,7 +327,7 @@ extern "C" int ark_concat_batches_device(int n, ArrowDeviceArray* ins, ArrowSche
     for (int i = 0; i < n; ++i) {
       ArrowDeviceArray view = ins[i];
       view.array = *(const ArrowArray*)owners[i].get();
-      bs.push_back(import_device(&view, &in_schemas[i], nullptr, owners[i]));
+      bs.push_back(import_device(&view, &in_schemas[i], nullptr, owners[i], true));
     }
     Batch r = concat_device(bs, lease.s);
     export_device(r, out, out_schema);
