@@ -10,14 +10,13 @@
 //     self-checked by scripts/gen_ryu_tables.py), positional with at least ".0" while the scientific
 //     exponent is in [-5, 9], d.ddde±x outside; NaN / ±inf → null.
 // Two passes, one thread per row: measure → exclusive scan → write.
-#include <cub/device/device_scan.cuh>
-
 #include <algorithm>
 
 #include "engine.h"
 #include "stage_store.cuh"
 #include "json_mini.h"
 #include "ryu_tables.h"
+#include "varlen.h"
 
 namespace ark {
 
@@ -275,7 +274,7 @@ __global__ void arrow_to_json_measure_kernel(const __grid_constant__ AjParams P,
   const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (r < P.n_rows) {
     const unsigned len = emit_row<true>(P, r, nullptr);
-    lens[r] = len < AJ_PAST_INT32 ? (int32_t)len : -1;  // a row past 2^31 - 1 bytes: pb_check_total counts it as too long
+    lens[r] = len < AJ_PAST_INT32 ? (int32_t)len : -1;  // a row past 2^31 - 1 bytes: varlen_guard counts it as too long
   }
 }
 // The lines of one CTA's rows are contiguous in the output: each thread formats its row into a shared-memory
@@ -354,7 +353,7 @@ Batch arrow_to_json_device(const Processor& proc, Batch& in, cudaStream_t stream
   P.n_rows = n;
   // A bound on the output bytes: per row the braces, each column's key and comma and its widest value ("-9223372036854775808",
   // "-1.2345678901234567e-308", "false", a string's quotes); a Utf8 byte becomes at most 6 ("\u00xx"), a Binary byte 2.
-  // While it stays below 2^31 the exact 64-bit sum in pb_check_total is skipped.
+  // While it stays below 2^31 the exact 64-bit sum in varlen_guard is skipped.
   int64_t row_bound = 2, var_bound = 0;
   for (auto& c : in.cols) {
     if (!c.present && c.field.format != "n") fail(ARK_ERR_UNSUPPORTED, "arrow_to_json: column '" + c.field.name + "' has Arrow type '" + c.field.format + "'");
@@ -374,30 +373,18 @@ Batch arrow_to_json_device(const Processor& proc, Batch& in, cudaStream_t stream
   }
   if (ap.has_include && P.n_cols == 0 && n > 0) fail_filtered_to_no_columns();
   const int64_t bound = var_bound < 0 ? -1 : var_bound + n * row_bound;
-  BufferPtr lens = device_alloc((size_t)(n + 1) * 4), offs = device_alloc((size_t)(n + 1) * 4);
+  BufferPtr lens = device_alloc((size_t)(n + 1) * 4);
   ARK_CUDA(cudaMemsetAsync(lens.get(), 0, (size_t)(n + 1) * 4, stream));
   const unsigned grid = (unsigned)std::max<int64_t>(1, ceil_div(n, 128));
   if (n) {
     KernelTimer t("arrow_to_json_measure_kernel", stream);
     arrow_to_json_measure_kernel<<<grid, 128, 0, stream>>>(P, (int32_t*)lens.get());
   }
-  // the int32 scan below wraps past 2^31 - 1 (and past 2^32 looks valid again): an output that does not fit fails first
-  pb_check_total((const int32_t*)lens.get(), n, bound, "Arrow JSON Serialization error: arrow_to_json output", stream);
-  size_t tb = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, tb, (int32_t*)lens.get(), (int32_t*)offs.get(), (int)(n + 1), stream);
-  BufferPtr tmp = device_alloc(tb + 16);
-  note_launch("cub::DeviceScan::ExclusiveSum");
-  cub::DeviceScan::ExclusiveSum(tmp.get(), tb, (int32_t*)lens.get(), (int32_t*)offs.get(), (int)(n + 1), stream);
-  BufferPtr h = pinned_alloc(64);
-  ARK_CUDA(cudaMemcpyAsync(h.get(), (int32_t*)offs.get() + n, 4, cudaMemcpyDeviceToHost, stream));
-  ARK_CUDA(cudaStreamSynchronize(stream));
-  const int32_t total = *(int32_t*)h.get();
-  BufferPtr bytes = device_alloc((size_t)total + 16);
+  const Varlen out_v = varlen_layout((const int32_t*)lens.get(), n, nullptr, bound, "Arrow JSON Serialization error: arrow_to_json output", stream);
   if (n) {
     KernelTimer t("arrow_to_json_write_kernel", stream);
-    // staging window: the average CTA's bytes + 50 %; CTAs whose rows are longer take the direct path
-    const int stage = (int)std::min<int64_t>(44 * 1024, round_up((int64_t)((double)total / (double)n * AJ_THREADS * 1.5) + 256, 1024));
-    arrow_to_json_write_kernel<<<grid, AJ_THREADS, stage, stream>>>(P, (const int32_t*)offs.get(), (uint8_t*)bytes.get(), stage);
+    const int stage = stage_window(out_v.total, n, AJ_THREADS);
+    arrow_to_json_write_kernel<<<grid, AJ_THREADS, stage, stream>>>(P, (const int32_t*)out_v.offsets.get(), (uint8_t*)out_v.bytes.get(), stage);
   }
   ARK_CUDA(cudaGetLastError());
   Batch out;
@@ -406,8 +393,7 @@ Batch arrow_to_json_device(const Processor& proc, Batch& in, cudaStream_t stream
   Column v;
   v.field.name = "__value__"; v.field.type = DType::Binary; v.field.nullable = false; v.field.format = "z";
   v.length = n;
-  v.offsets = (const int32_t*)offs.get(); v.data = (const uint8_t*)bytes.get(); v.data_bytes = total; v.first_offset = 0;
-  v.owners = {offs, bytes};
+  set_varlen(v, out_v);
   out.cols.push_back(v);
   ARK_CUDA(cudaStreamSynchronize(stream));
   return out;

@@ -11,8 +11,8 @@
 //   avro_decode_kernel  one thread per record (the records of a CTA arrive in shared memory by one 1-D TMA bulk copy):
 //                       fixed-width values and validity go to their rows, string / bytes record their spans, and strings
 //                       are checked for UTF-8 in the same pass;
-//   strings             exclusive scan of the span lengths, then protobuf.cu's span copy (pb_scan / pb_check_total /
-//                       launch_span_copy: the same 2 GiB int32-offset guard).
+//   strings             exclusive scan of the span lengths behind the 2 GiB int32-offset guard, then a span copy
+//                       (varlen.cu's varlen_guard / varlen_scan / launch_span_copy).
 // Schema: a record whose fields are null, boolean, int, long, float, double, bytes or string, or a two-branch union of
 // null and one of these in either order → Null, Boolean, Int32, Int64, Float32, Float64, Binary, Utf8 (DataFusion's Avro
 // reader's mapping); a plain field is non-nullable, a union field nullable.  Anything else (nested record, array, map,
@@ -29,8 +29,6 @@
 //     (0-based in the file) and its block's offset.  Within a record the first failing field in order decides the text.
 //     A snappy or CRC failure is the failure of its block's first record.
 // oracle/avro_oracle.py restates all of this in Python; tests/test_avro_input_gpu.py compares the two.
-#include <cub/device/device_scan.cuh>
-
 #include <algorithm>
 #include <cstdio>
 
@@ -38,6 +36,7 @@
 #include "json_mini.h"
 #include "tma.cuh"
 #include "utf8.cuh"
+#include "varlen.h"
 
 namespace ark {
 
@@ -694,7 +693,7 @@ Batch avro_batch(AvroFile& f, const BufferPtr& file_dev, int64_t r0, int64_t n, 
     ARK_CUDA(cudaStreamSynchronize(stream));
     error_check();
     for (size_t k = 0; k < nf; ++k)
-      if (lens[k]) pb_check_total((const int32_t*)lens[k].get(), n, bound, "avro input: column '" + f.fields[k].name + "'", stream);
+      if (lens[k]) varlen_guard((const int32_t*)lens[k].get(), n, bound, "avro input: column '" + f.fields[k].name + "'", stream);
   }
   // the error word, every string total and every null count come back in one round trip
   std::vector<BufferPtr> offs(nf), vbits(nf), bits(nf);
@@ -703,7 +702,7 @@ Batch avro_batch(AvroFile& f, const BufferPtr& file_dev, int64_t r0, int64_t n, 
   ARK_CUDA(cudaMemcpyAsync(h.get(), err.get(), 8, cudaMemcpyDeviceToHost, stream));
   for (size_t k = 0; k < nf; ++k) {
     if (lens[k]) {
-      offs[k] = pb_scan((const int32_t*)lens[k].get(), n, stream);
+      offs[k] = varlen_scan((const int32_t*)lens[k].get(), n, stream);
       ARK_CUDA(cudaMemcpyAsync((char*)h.get() + 8 + 16 * k, (int32_t*)offs[k].get() + n, 4, cudaMemcpyDeviceToHost, stream));
     }
     if (valid[k]) {
@@ -728,9 +727,8 @@ Batch avro_batch(AvroFile& f, const BufferPtr& file_dev, int64_t r0, int64_t n, 
     if (offs[k]) {
       const int32_t total = *(const int32_t*)((char*)h.get() + 8 + 16 * k);
       BufferPtr bytes = device_alloc((size_t)total + 16);
-      if (total) launch_span_copy(P.arena, (const long long*)src[k].get(), (const int32_t*)offs[k].get(), n, (uint8_t*)bytes.get(), stream);
-      c.offsets = (const int32_t*)offs[k].get(); c.data = (const uint8_t*)bytes.get(); c.data_bytes = total; c.first_offset = 0;
-      c.owners = {offs[k], bytes};
+      if (total) launch_span_copy(P.arena, nullptr, (const long long*)src[k].get(), (const int32_t*)offs[k].get(), n, (uint8_t*)bytes.get(), stream);
+      set_varlen(c, {offs[k], bytes, total});
     } else if (t == DType::Bool) {
       BufferPtr bb = device_alloc((size_t)(n + 7) / 8 + 1);
       launch_pack_bits((const uint8_t*)values[k].get(), n, (uint8_t*)bb.get(), nullptr, stream);

@@ -98,12 +98,6 @@ const std::string& protobuf_to_arrow_value_field(const Processor& p);
 Batch protobuf_to_arrow_device(const Processor& proc, Batch& in, cudaStream_t stream);
 std::unique_ptr<Processor> make_arrow_to_protobuf(const char* config_json);
 Batch arrow_to_protobuf_device(const Processor& proc, Batch& in, cudaStream_t stream);
-// protobuf.cu: exclusive scan of n + 1 int32 lengths into a column's offsets; the guard that fails with Process when the
-// lengths add up past a Binary / Utf8 column's 2 GiB (checked exactly only when `bound` does not rule it out); the copy
-// of each row's span of `data` into the column's bytes
-BufferPtr pb_scan(const int32_t* lens, int64_t n, cudaStream_t stream);
-void pb_check_total(const int32_t* lens, int64_t n, int64_t bound, const std::string& what, cudaStream_t stream);
-void launch_span_copy(const uint8_t* data, const long long* src, const int32_t* offsets, int64_t n_rows, uint8_t* out, cudaStream_t stream);
 // avro.cu: the `file` input's Avro object container files
 struct AvroFile;
 std::shared_ptr<AvroFile> avro_open(const std::string& path);  // header, schema and codec (nullptr: cannot open)

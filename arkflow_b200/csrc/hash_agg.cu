@@ -9,13 +9,13 @@
 // a probe reads a whole bucket, a key is claimed with a single 128-bit CAS (ATOMG.CAS.128), accumulators take
 // fire-and-forget RED atomics; a warp whose lanes all hit the same group reduces with shuffles first.
 // Algorithmic traffic = key + argument bytes read once (SURVEY.md §8(d): 24 B/row for config 3).
-#include <cub/device/device_scan.cuh>
 
 #include "agg_acc.cuh"
 #include "engine.h"
 #include "group_exchange.h"
 #include "hash_agg.cuh"
 #include "hashkey.cuh"
+#include "varlen.h"
 #include "vm.cuh"
 
 namespace ark {
@@ -528,9 +528,10 @@ static void compact_groups(DenseGroups& dg, const ColView& kc, int key_kind, int
 }
 
 // key column of the dense groups
-// kc: the column long keys (> 12 bytes) point into; may_null: emit a validity bitmap
+// kc: the column long keys (> 12 bytes) point into; may_null: emit a validity bitmap; key_bytes: a bound on the string
+// keys' total bytes (< 0: none)
 static Column emit_key_column(const AggExec& ex, const DenseGroups& dg, const ColView& kc, bool may_null, const std::string& name,
-                              bool nullable, cudaStream_t stream) {
+                              bool nullable, int64_t key_bytes, cudaStream_t stream) {
   const unsigned int G = dg.n_groups;
   Column c;
   c.field.name = name; c.field.type = ex.key_type; c.field.nullable = nullable; c.length = G;
@@ -540,29 +541,19 @@ static Column emit_key_column(const AggExec& ex, const DenseGroups& dg, const Co
   const int kstride = dg.stride;
   const unsigned int* slots = (const unsigned int*)dg.slots.get();
   if (ex.key_kind == KEY_BYTES) {
-    BufferPtr lens = device_alloc((size_t)(G + 1) * 4), offs = device_alloc((size_t)(G + 1) * 4);
+    BufferPtr lens = device_alloc((size_t)(G + 1) * 4);
     ARK_CUDA(cudaMemsetAsync(lens.get(), 0, (size_t)(G + 1) * 4, stream));
     if (G) {
       KernelTimer t("agg_key_lengths_kernel", stream);
       agg_key_lengths_kernel<<<grid, 256, 0, stream>>>(keys, kstride, slots, G, (int32_t*)lens.get());
     }
-    size_t tmp_bytes = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, (int32_t*)lens.get(), (int32_t*)offs.get(), (int)(G + 1), stream);
-    BufferPtr tmp = device_alloc(tmp_bytes + 16);
-    note_launch("cub::DeviceScan::ExclusiveSum");
-    cub::DeviceScan::ExclusiveSum(tmp.get(), tmp_bytes, (int32_t*)lens.get(), (int32_t*)offs.get(), (int)(G + 1), stream);
-    BufferPtr h = pinned_alloc(64);
-    ARK_CUDA(cudaMemcpyAsync(h.get(), (int32_t*)offs.get() + G, 4, cudaMemcpyDeviceToHost, stream));
-    ARK_CUDA(cudaStreamSynchronize(stream));
-    const int32_t total = *(int32_t*)h.get();
-    BufferPtr bytes = device_alloc((size_t)total + 16);
+    const Varlen v = varlen_layout((const int32_t*)lens.get(), G, nullptr, key_bytes, "GROUP BY key column '" + name + "'", stream);
     if (G) {
       KernelTimer t("agg_emit_keys_kernel", stream);
-      agg_emit_keys_kernel<<<grid, 256, 0, stream>>>(keys, kstride, slots, G, kc, ex.key_kind, nullptr, nullptr, (const int32_t*)offs.get(),
-                                                     (uint8_t*)bytes.get(), (uint8_t*)valid_bytes.get());
+      agg_emit_keys_kernel<<<grid, 256, 0, stream>>>(keys, kstride, slots, G, kc, ex.key_kind, nullptr, nullptr, (const int32_t*)v.offsets.get(),
+                                                     (uint8_t*)v.bytes.get(), (uint8_t*)valid_bytes.get());
     }
-    c.offsets = (const int32_t*)offs.get(); c.data = (const uint8_t*)bytes.get(); c.data_bytes = total; c.first_offset = 0;
-    c.owners = {offs, bytes};
+    set_varlen(c, v);
   } else if (ex.key_kind == KEY_INT64) {
     BufferPtr vals = device_alloc((size_t)std::max<unsigned int>(G, 1) * 8);
     if (G) {
@@ -590,9 +581,10 @@ static Column emit_key_column(const AggExec& ex, const DenseGroups& dg, const Co
   return c;
 }
 
+// each group's key is the key of one input row, so the key column's bytes bound the output's
 static Column emit_key_column(const AggExec& ex, const DenseGroups& dg, const Column& src, const std::string& name,
                               bool nullable, cudaStream_t stream) {
-  return emit_key_column(ex, dg, src.view(), src.validity != nullptr, name, nullable, stream);
+  return emit_key_column(ex, dg, src.view(), src.validity != nullptr, name, nullable, varlen_bytes_bound(src), stream);
 }
 
 // pair keys: the row each group was first seen at (Key16.lo) → gather index for take_column
@@ -938,7 +930,8 @@ bool run_group_by_merge(const Plan& plan, DistCtx& d, Batch& out, cudaStream_t s
   for (const PostItem& pi : plan.post) {
     if (pi.kind == PostItem::Key) {
       const Field& kf = plan.input_fields[plan.used_cols[plan.keys[0].slot]];
-      out.cols.push_back(emit_key_column(mx, dg, ColView{}, kf.nullable, pi.name, kf.nullable, stream));
+      // every key arrived inline (at most 12 bytes): the exchange does not carry longer ones
+      out.cols.push_back(emit_key_column(mx, dg, ColView{}, kf.nullable, pi.name, kf.nullable, (int64_t)G * 12, stream));
     } else if (pi.kind == PostItem::Agg) {
       const AggOutput& o = outs[pi.index];
       const AggSpec& sp = plan.aggs[pi.index];

@@ -17,6 +17,7 @@
 #include "engine.h"
 #include "hashkey.cuh"
 #include "stage_store.cuh"
+#include "varlen.h"
 
 namespace ark {
 
@@ -203,7 +204,6 @@ __device__ __forceinline__ void gather_string(uint8_t* dst, const uint8_t* src, 
 }
 
 constexpr int TAKE_TILE = 1024;
-constexpr int TAKE_STAGE_MAX = 44 * 1024;  // most bytes of output staged per tile; longer tiles take the per-row path
 
 // Gathers the bytes of TAKE_TILE output rows into shared memory (their output range is contiguous), then
 // writes the range with destination-aligned 16-byte stores.  Replaces the warp-per-row kernel on the join's
@@ -304,6 +304,8 @@ int key_kind_of(DType t) {
   }
 }
 
+const char* const OFFSET_OVERFLOW = "Collection query results error: Arrow error: offset overflow, result column exceeds 2 GiB";
+
 unsigned grid_for(int64_t n, int threads = 256) { return (unsigned)std::max<int64_t>(1, std::min<int64_t>(ceil_div(n, threads), sm_count() * 16)); }
 
 }  // namespace
@@ -331,29 +333,17 @@ Column take_column(const Column& src, const unsigned int* idx, int64_t n, const 
     }
     case DType::Utf8: case DType::Binary: {
       // lens[n] = 0 closes the scan; the 64-bit total sits in the 8 bytes after it
-      BufferPtr lens = device_alloc((size_t)(n + 1) * 4 + 16), offs = device_alloc((size_t)(n + 1) * 4);
+      BufferPtr lens = device_alloc((size_t)(n + 1) * 4 + 16);
       ARK_CUDA(cudaMemsetAsync(lens.get(), 0, (size_t)(n + 1) * 4 + 16, stream));
       unsigned long long* total64 = (unsigned long long*)((uint8_t*)lens.get() + round_up((int64_t)(n + 1) * 4, 8));
       if (n) { KernelTimer t("take_lengths_kernel", stream); take_lengths_kernel<<<g, 256, 0, stream>>>(src.offsets, idx, n, (int32_t*)lens.get(), total64); }
-      size_t tb = 0;
-      cub::DeviceScan::ExclusiveSum(nullptr, tb, (int32_t*)lens.get(), (int32_t*)offs.get(), (int)(n + 1), stream);
-      BufferPtr tmp = device_alloc(tb + 16);
-      note_launch("cub::DeviceScan::ExclusiveSum");
-      cub::DeviceScan::ExclusiveSum(tmp.get(), tb, (int32_t*)lens.get(), (int32_t*)offs.get(), (int)(n + 1), stream);
-      BufferPtr h = pinned_alloc(64);
-      ARK_CUDA(cudaMemcpyAsync(h.get(), total64, 8, cudaMemcpyDeviceToHost, stream));
-      ARK_CUDA(cudaStreamSynchronize(stream));
-      const unsigned long long total64_h = *(const unsigned long long*)h.get();
-      if (total64_h > 2147483647ull) fail(ARK_ERR_PROCESS, "Collection query results error: Arrow error: offset overflow, result column exceeds 2 GiB");
-      const int32_t total = (int32_t)total64_h;  // = offs[n]: the scan did not wrap
-      BufferPtr bytes = device_alloc((size_t)total + 16);
+      const Varlen v = varlen_layout((const int32_t*)lens.get(), n, total64, -1, OFFSET_OVERFLOW, stream);
       if (n) {
         KernelTimer t("take_bytes_tile_kernel", stream);
-        const int stage = (int)std::min<int64_t>(TAKE_STAGE_MAX, round_up((int64_t)((double)total / (double)n * TAKE_TILE * 1.5) + 256, 1024));
-        take_bytes_tile_kernel<<<(unsigned)ceil_div(n, TAKE_TILE), 256, stage, stream>>>(src.data, src.offsets, idx, n, (const int32_t*)offs.get(), (uint8_t*)bytes.get(), stage);
+        const int stage = stage_window(v.total, n, TAKE_TILE);
+        take_bytes_tile_kernel<<<(unsigned)ceil_div(n, TAKE_TILE), 256, stage, stream>>>(src.data, src.offsets, idx, n, (const int32_t*)v.offsets.get(), (uint8_t*)v.bytes.get(), stage);
       }
-      c.offsets = (const int32_t*)offs.get(); c.data = (const uint8_t*)bytes.get(); c.data_bytes = total; c.first_offset = 0;
-      c.owners = {offs, bytes};
+      set_varlen(c, v);
       break;
     }
     default:
@@ -392,7 +382,8 @@ std::vector<Column> take_columns(const std::vector<TakeSpec>& specs, const unsig
   TakeMultiParams P;
   memset(&P, 0, sizeof P);
   P.idx[0] = idx0; P.idx[1] = idx1;
-  std::vector<BufferPtr> fbuf, lens, offs;
+  std::vector<BufferPtr> fbuf, lens;
+  std::vector<Varlen> strv(strs.size());
   // each string column's 64-bit byte total: added up by take_multi_kernel, fetched in one round trip
   BufferPtr sums = device_alloc(8 * (size_t)std::max<size_t>(strs.size(), 1)), h = pinned_alloc(8 * (size_t)std::max<size_t>(strs.size(), 1));
   if (!strs.empty()) ARK_CUDA(cudaMemsetAsync(sums.get(), 0, 8 * strs.size(), stream));
@@ -403,10 +394,10 @@ std::vector<Column> take_columns(const std::vector<TakeSpec>& specs, const unsig
     ++P.n_fixed; fbuf.push_back(d);
   }
   for (int k : strs) {
-    BufferPtr l = device_alloc((size_t)(n + 1) * 4), o = device_alloc((size_t)(n + 1) * 4);
+    BufferPtr l = device_alloc((size_t)(n + 1) * 4);
     ARK_CUDA(cudaMemsetAsync((int32_t*)l.get() + n, 0, 4, stream));
     P.soff[P.n_str] = specs[k].src->offsets; P.slen[P.n_str] = (int32_t*)l.get(); P.sside[P.n_str] = (uint8_t)specs[k].side;
-    ++P.n_str; lens.push_back(l); offs.push_back(o);
+    ++P.n_str; lens.push_back(l);
   }
   {
     KernelTimer t("take_multi_kernel", stream);
@@ -414,30 +405,23 @@ std::vector<Column> take_columns(const std::vector<TakeSpec>& specs, const unsig
   }
   // string columns: offsets by scan; every column's total comes back in one round trip
   if (!strs.empty()) ARK_CUDA(cudaMemcpyAsync(h.get(), sums.get(), 8 * strs.size(), cudaMemcpyDeviceToHost, stream));
-  for (size_t j = 0; j < strs.size(); ++j) {
-    size_t tb = 0;
-    cub::DeviceScan::ExclusiveSum(nullptr, tb, (int32_t*)lens[j].get(), (int32_t*)offs[j].get(), (int)(n + 1), stream);
-    BufferPtr tmp = device_alloc(tb + 16);
-    note_launch("cub::DeviceScan::ExclusiveSum");
-    cub::DeviceScan::ExclusiveSum(tmp.get(), tb, (int32_t*)lens[j].get(), (int32_t*)offs[j].get(), (int)(n + 1), stream);
-  }
+  for (size_t j = 0; j < strs.size(); ++j) strv[j].offsets = varlen_scan((const int32_t*)lens[j].get(), n, stream);
   if (!strs.empty()) ARK_CUDA(cudaStreamSynchronize(stream));
   for (size_t j = 0; j < strs.size(); ++j) {
-    const unsigned long long total64 = ((const unsigned long long*)h.get())[j];
-    if (total64 > 2147483647ull) fail(ARK_ERR_PROCESS, "Collection query results error: Arrow error: offset overflow, result column exceeds 2 GiB");
-    const int32_t total = (int32_t)total64;  // = offs[j][n]: the scan did not wrap
+    Varlen& v = strv[j];
+    v.total = varlen_guard(((const unsigned long long*)h.get())[j], OFFSET_OVERFLOW);
+    v.bytes = device_alloc((size_t)v.total + 16);
     const TakeSpec& sp = specs[strs[j]];
-    BufferPtr bytes = device_alloc((size_t)total + 16);
     {
       KernelTimer t("take_bytes_tile_kernel", stream);
-      const int stage = (int)std::min<int64_t>(TAKE_STAGE_MAX, round_up((int64_t)((double)total / (double)n * TAKE_TILE * 1.5) + 256, 1024));
-      take_bytes_tile_kernel<<<(unsigned)ceil_div(n, TAKE_TILE), 256, stage, stream>>>(sp.src->data, sp.src->offsets, sp.side == 0 ? idx0 : idx1, n, (const int32_t*)offs[j].get(),
-                                                                                      (uint8_t*)bytes.get(), stage);
+      const int stage = stage_window(v.total, n, TAKE_TILE);
+      take_bytes_tile_kernel<<<(unsigned)ceil_div(n, TAKE_TILE), 256, stage, stream>>>(sp.src->data, sp.src->offsets, sp.side == 0 ? idx0 : idx1, n, (const int32_t*)v.offsets.get(),
+                                                                                      (uint8_t*)v.bytes.get(), stage);
     }
     Column& c = out[strs[j]];
     c.field = sp.src->field; c.field.name = sp.name; c.length = n;
-    c.offsets = (const int32_t*)offs[j].get(); c.data = (const uint8_t*)bytes.get(); c.data_bytes = total; c.first_offset = 0;
-    c.owners = {offs[j], bytes}; c.validity = nullptr; c.null_count = 0;
+    set_varlen(c, v);
+    c.validity = nullptr; c.null_count = 0;
   }
   for (size_t j = 0; j < fixed.size(); ++j) {
     const TakeSpec& sp = specs[fixed[j]];

@@ -40,7 +40,6 @@
 
 #include <thrust/iterator/counting_iterator.h>
 
-#include <cub/device/device_scan.cuh>
 #include <cub/device/device_select.cuh>
 
 #include <thrust/count.h>
@@ -50,6 +49,7 @@
 #include "engine.h"
 #include "json_mini.h"
 #include "utf8.cuh"
+#include "varlen.h"
 
 using namespace ark;
 
@@ -555,24 +555,14 @@ Batch csv_batch(ark_input* in, int64_t l0, int64_t n, cudaStream_t stream) {
         break;
       }
       default: {
-        BufferPtr offs = device_alloc((size_t)(n + 1) * 4);
-        size_t tb = 0;
-        cub::DeviceScan::ExclusiveSum(nullptr, tb, (int32_t*)slen[c].get(), (int32_t*)offs.get(), (int)(n + 1), stream);
-        BufferPtr tmp = device_alloc(tb + 16);
-        note_launch("cub::DeviceScan::ExclusiveSum");
-        cub::DeviceScan::ExclusiveSum(tmp.get(), tb, (int32_t*)slen[c].get(), (int32_t*)offs.get(), (int)(n + 1), stream);
-        BufferPtr ht = pinned_alloc(16);
-        ARK_CUDA(cudaMemcpyAsync(ht.get(), (int32_t*)offs.get() + n, 4, cudaMemcpyDeviceToHost, stream));
-        ARK_CUDA(cudaStreamSynchronize(stream));
-        const int32_t total = *(int32_t*)ht.get();
-        BufferPtr bytes = device_alloc((size_t)std::max(total, 0) + 16);
+        // a field's bytes lie inside its line, so the batch's byte span (at most 2 GiB, checked above) bounds the column
+        const Varlen v = varlen_layout((const int32_t*)slen[c].get(), n, nullptr, byte1 - byte0, "file input: column '" + in->csv_names[c] + "'", stream);
         if (n) {
           KernelTimer t("csv_strings_kernel", stream);
-          csv_strings_kernel<<<grid_of(n), 256, 0, stream>>>(P.data, n, (const int32_t*)offs.get(), (const long long*)ssrc[c].get(), (const int32_t*)sraw[c].get(), (uint8_t*)bytes.get());
+          csv_strings_kernel<<<grid_of(n), 256, 0, stream>>>(P.data, n, (const int32_t*)v.offsets.get(), (const long long*)ssrc[c].get(), (const int32_t*)sraw[c].get(), (uint8_t*)v.bytes.get());
         }
         col.field.type = DType::Utf8; col.field.format = "u";
-        col.offsets = (const int32_t*)offs.get(); col.data = (const uint8_t*)bytes.get(); col.data_bytes = total; col.first_offset = 0;
-        col.owners = {offs, bytes};
+        set_varlen(col, v);
         break;
       }
     }

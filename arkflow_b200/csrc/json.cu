@@ -23,6 +23,7 @@
 #include "json_mini.h"
 #include "decimal.cuh"
 #include "utf8.cuh"
+#include "varlen.h"
 
 namespace ark {
 
@@ -778,20 +779,10 @@ void alloc_field(DType type, int64_t rows, FieldBufs& fb, JsonField& F, cudaStre
   }
 }
 
-// exclusive scan of n + 1 int32 lengths; returns the offsets buffer, *total_dev points at the last entry
-BufferPtr scan_lengths(const int32_t* lens, int64_t n, cudaStream_t stream) {
-  BufferPtr offs = device_alloc((size_t)(n + 1) * 4);
-  size_t tb = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, tb, lens, (int32_t*)offs.get(), (int)(n + 1), stream);
-  BufferPtr t2 = device_alloc(tb + 16);
-  note_launch("cub::DeviceScan::ExclusiveSum");
-  cub::DeviceScan::ExclusiveSum(t2.get(), tb, lens, (int32_t*)offs.get(), (int)(n + 1), stream);
-  return offs;
-}
-
 // Finishes a scalar column whose decode pass has run: validity bitmap, Boolean bit packing, string bytes.
-// `data` is the byte base str_src refers to.  Synchronises the stream (string totals / null counts).
-Column finish_scalar(const std::string& name, DType type, int64_t rows, FieldBufs& fb, const uint8_t* data, cudaStream_t stream) {
+// `data` is the byte base str_src refers to, `data_bytes` the bytes of the input Binary column there.  Synchronises the
+// stream (string totals / null counts).
+Column finish_scalar(const std::string& name, DType type, int64_t rows, FieldBufs& fb, const uint8_t* data, int64_t data_bytes, cudaStream_t stream) {
   Column c;
   c.field.name = name; c.field.type = type; c.field.nullable = true; c.length = rows;
   if (type == DType::Null) { c.field.format = "n"; return c; }
@@ -803,7 +794,9 @@ Column finish_scalar(const std::string& name, DType type, int64_t rows, FieldBuf
   }
   ARK_CUDA(cudaMemcpyAsync(h.get(), nulls.get(), 8, cudaMemcpyDeviceToHost, stream));
   if (type == DType::Utf8) {
-    fb.str_offsets = scan_lengths((const int32_t*)fb.str_len.get(), rows, stream);
+    // a decoded string is never longer than its raw span inside the input column
+    varlen_guard((const int32_t*)fb.str_len.get(), rows, data_bytes, "json_to_arrow: column '" + name + "'", stream);
+    fb.str_offsets = varlen_scan((const int32_t*)fb.str_len.get(), rows, stream);
     ARK_CUDA(cudaMemcpyAsync((char*)h.get() + 8, (int32_t*)fb.str_offsets.get() + rows, 4, cudaMemcpyDeviceToHost, stream));
   }
   ARK_CUDA(cudaStreamSynchronize(stream));
@@ -821,8 +814,7 @@ Column finish_scalar(const std::string& name, DType type, int64_t rows, FieldBuf
       json_strings_kernel<<<(unsigned)ceil_div(rows, 256), 256, 0, stream>>>(data, (const long long*)fb.str_src.get(), (const int32_t*)fb.str_raw.get(),
                                                                             (const int32_t*)fb.str_offsets.get(), rows, (uint8_t*)bytes.get());
     }
-    c.offsets = (const int32_t*)fb.str_offsets.get(); c.data = (const uint8_t*)bytes.get(); c.data_bytes = total; c.first_offset = 0;
-    c.owners = {fb.str_offsets, bytes};
+    set_varlen(c, {fb.str_offsets, bytes, total});
   }
   const long long n_null = *(const long long*)h.get();
   if (rows > 0 && n_null > 0) { c.validity = (const uint8_t*)fb.vbits.get(); c.null_count = n_null; c.owners.push_back(fb.vbits); }
@@ -834,7 +826,7 @@ Column finish_scalar(const std::string& name, DType type, int64_t rows, FieldBuf
 }
 
 // List<primitive> column from the raw spans of its rows (fb.str_src / fb.str_raw hold them, fb.valid_bytes the row validity)
-Column finish_list(const InferredField& f, int64_t rows, FieldBufs& fb, const uint8_t* data, cudaStream_t stream) {
+Column finish_list(const InferredField& f, int64_t rows, FieldBufs& fb, const uint8_t* data, int64_t data_bytes, cudaStream_t stream) {
   BufferPtr err = device_alloc(16), h = pinned_alloc(32);
   ARK_CUDA(cudaMemsetAsync(err.get(), 0, 16, stream));
   BufferPtr counts = device_alloc((size_t)(rows + 1) * 4);
@@ -844,7 +836,9 @@ Column finish_list(const InferredField& f, int64_t rows, FieldBufs& fb, const ui
     KernelTimer t("json_list_count_kernel", stream);
     json_list_count_kernel<<<g, 128, 0, stream>>>(data, (const long long*)fb.str_src.get(), (const int32_t*)fb.str_raw.get(), rows, (int32_t*)counts.get(), (int32_t*)err.get());
   }
-  BufferPtr offs = scan_lengths((const int32_t*)counts.get(), rows, stream);
+  // every element takes at least one byte of its row's raw span inside the input column
+  varlen_guard((const int32_t*)counts.get(), rows, data_bytes, "json_to_arrow: column '" + f.name + "'", stream);
+  BufferPtr offs = varlen_scan((const int32_t*)counts.get(), rows, stream);
   ARK_CUDA(cudaMemcpyAsync(h.get(), (int32_t*)offs.get() + rows, 4, cudaMemcpyDeviceToHost, stream));
   ARK_CUDA(cudaMemcpyAsync((char*)h.get() + 8, err.get(), 8, cudaMemcpyDeviceToHost, stream));
   ARK_CUDA(cudaStreamSynchronize(stream));
@@ -862,7 +856,7 @@ Column finish_list(const InferredField& f, int64_t rows, FieldBufs& fb, const ui
   ARK_CUDA(cudaMemcpyAsync((char*)h.get() + 8, err.get(), 8, cudaMemcpyDeviceToHost, stream));
   ARK_CUDA(cudaStreamSynchronize(stream));
   if (((int32_t*)((char*)h.get() + 8))[0]) raise_json(((int32_t*)((char*)h.get() + 8))[0], ((int32_t*)((char*)h.get() + 8))[1], "row");
-  Column child = finish_scalar("item", f.elem, total, cb, data, stream);  // arrow-rs names a list's field "item"
+  Column child = finish_scalar("item", f.elem, total, cb, data, data_bytes, stream);  // arrow-rs names a list's field "item"
   Column c;
   c.field.name = f.name; c.field.type = DType::List; c.field.format = "+l"; c.field.nullable = true; c.length = rows;
   // row validity
@@ -950,7 +944,7 @@ struct FieldTable {
 // optimistic: payload i → row i in ONE pass; returns false (nothing raised) when the batch is not of that shape or
 // holds an error — the caller then takes the two-pass route, which reports errors the canonical way.
 bool decode_fields(const std::vector<InferredField>& specs, JsonParams Q, unsigned grid, size_t smem, int64_t rows, bool optimistic,
-                   const long long* row_start, const uint8_t* data, std::vector<Column>& out_cols, cudaStream_t stream) {
+                   const long long* row_start, const uint8_t* data, int64_t data_bytes, std::vector<Column>& out_cols, cudaStream_t stream) {
   const size_t nf = specs.size();
   std::vector<FieldBufs> fb(nf);
   std::vector<JsonField> table(nf);
@@ -1013,7 +1007,7 @@ bool decode_fields(const std::vector<InferredField>& specs, JsonParams Q, unsign
   out_cols.clear();
   for (size_t k = 0; k < nf; ++k) {
     const InferredField& f = specs[k];
-    if (f.type == DType::List) out_cols.push_back(finish_list(f, rows, fb[k], data, stream));
+    if (f.type == DType::List) out_cols.push_back(finish_list(f, rows, fb[k], data, data_bytes, stream));
     else if (f.type == DType::Struct) {
       // the struct's children: the same decoder over the captured spans, one row per span
       JsonParams S;
@@ -1022,8 +1016,8 @@ bool decode_fields(const std::vector<InferredField>& specs, JsonParams Q, unsign
       S.span_src = (const long long*)fb[k].str_src.get(); S.span_len = (const int32_t*)fb[k].str_raw.get();
       std::vector<Column> kids;
       if (rows > 0 && !f.kids.empty()) {
-        if (!decode_fields(f.kids, S, (unsigned)ceil_div(rows, JS_THREADS), 32, rows, true, nullptr, data, kids, stream))
-          decode_fields(f.kids, S, (unsigned)ceil_div(rows, JS_THREADS), 32, rows, false, nullptr, data, kids, stream);  // raises the canonical error
+        if (!decode_fields(f.kids, S, (unsigned)ceil_div(rows, JS_THREADS), 32, rows, true, nullptr, data, data_bytes, kids, stream))
+          decode_fields(f.kids, S, (unsigned)ceil_div(rows, JS_THREADS), 32, rows, false, nullptr, data, data_bytes, kids, stream);  // raises the canonical error
       } else {
         for (auto& kf : f.kids) { Column kc; kc.field.name = kf.name; kc.field.type = kf.type; kc.field.nullable = true; kc.length = rows; if (kf.type == DType::Null) kc.field.format = "n"; kids.push_back(kc); }
       }
@@ -1041,7 +1035,7 @@ bool decode_fields(const std::vector<InferredField>& specs, JsonParams Q, unsign
       }
       c.children = std::move(kids);
       out_cols.push_back(std::move(c));
-    } else out_cols.push_back(finish_scalar(f.name, f.type, rows, fb[k], data, stream));
+    } else out_cols.push_back(finish_scalar(f.name, f.type, rows, fb[k], data, data_bytes, stream));
   }
   ARK_CUDA(cudaGetLastError());
   ARK_CUDA(cudaStreamSynchronize(stream));
@@ -1118,7 +1112,7 @@ Batch json_to_arrow_device(const Processor& proc, Batch& in, cudaStream_t stream
 
   // ---- one pass when every payload holds exactly one record (the shape of every shipped example) ----
   static const bool two_pass_only = getenv("ARK_JSON_TWO_PASS") != nullptr;
-  if (!two_pass_only && decode_fields(fields, P, grid, smem, n, true, nullptr, col.data, out.cols, stream)) { out.num_rows = n; return out; }
+  if (!two_pass_only && decode_fields(fields, P, grid, smem, n, true, nullptr, col.data, col.data_bytes, out.cols, stream)) { out.num_rows = n; return out; }
 
   // ---- general route: records per payload → row offsets → parse ----
   BufferPtr err = device_alloc(16), h = pinned_alloc(64);
@@ -1145,7 +1139,7 @@ Batch json_to_arrow_device(const Processor& proc, Batch& in, cudaStream_t stream
   ARK_CUDA(cudaStreamSynchronize(stream));
   if (((const int32_t*)h.get())[0] != JE_NONE) raise_json(((const int32_t*)h.get())[0], ((const int32_t*)h.get())[1], "payload");
   const int64_t rows = *(const long long*)((char*)h.get() + 16);
-  decode_fields(fields, P, grid, smem, rows, false, (const long long*)row_start.get(), col.data, out.cols, stream);
+  decode_fields(fields, P, grid, smem, rows, false, (const long long*)row_start.get(), col.data, col.data_bytes, out.cols, stream);
   out.num_rows = rows;
   return out;
 }

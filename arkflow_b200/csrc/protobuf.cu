@@ -33,8 +33,6 @@
 //     raises ARK_ERR_UNSUPPORTED, as in arrow_to_json.
 // Library limits, ARK_ERR_UNSUPPORTED: more than 64 fields in a decoded message, more than 64 encoded fields.  A string /
 // bytes column or an encoded message column of 2 GiB or more (int32 offsets) raises Process before anything is written.
-#include <cub/device/device_scan.cuh>
-
 #include <algorithm>
 
 #include "engine.h"
@@ -43,6 +41,7 @@
 #include "stage_store.cuh"
 #include "tma.cuh"
 #include "utf8.cuh"
+#include "varlen.h"
 
 namespace ark {
 
@@ -270,19 +269,6 @@ __global__ void protobuf_valid_kernel(const uint8_t* validity, int32_t bit0, int
   if (i < n) flags[i] = (validity[(i + bit0) >> 3] >> ((i + bit0) & 7)) & 1;
 }
 
-// string / bytes column bytes: thread per row, from the payload column or from the default blob
-__global__ void protobuf_strings_kernel(const uint8_t* data, const uint8_t* dflt, const long long* src, const int32_t* offsets,
-                                        int64_t n_rows, uint8_t* out) {
-  const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= n_rows) return;
-  const int len = offsets[r + 1] - offsets[r];
-  if (len == 0) return;
-  const long long s = src[r];
-  const uint8_t* from = s >= 0 ? data + s : dflt + (-1 - s);
-  uint8_t* d = out + offsets[r];
-  for (int k = 0; k < len; ++k) d[k] = from[k];
-}
-
 // ---- encode -----------------------------------------------------------------------------------------------------
 struct PbEncCol {
   uint8_t kind;      // PbKind
@@ -363,7 +349,7 @@ __global__ void protobuf_encode_measure_kernel(const __grid_constant__ PbEncPara
   const int64_t r = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (r < P.n_rows) {
     const long long len = pb_emit_row<true>(P, r, nullptr);
-    lens[r] = len <= INT32_MAX ? (int32_t)len : -1;  // a message past 2^31 - 1 bytes: pb_check_total counts it as too long
+    lens[r] = len <= INT32_MAX ? (int32_t)len : -1;  // a message past 2^31 - 1 bytes: varlen_guard counts it as too long
   }
 }
 
@@ -387,56 +373,6 @@ __global__ void __launch_bounds__(PB_THREADS, 8) protobuf_encode_write_kernel(co
   __syncthreads();
   stage_store(out + bb, pe_stage, mis, tb, threadIdx.x, PB_THREADS);
 }
-
-// Sum of n non-negative int32 lengths, accumulated in 64 bits.
-__global__ void protobuf_sum64_kernel(const int32_t* lens, int64_t n, unsigned long long* total) {
-  long long acc = 0;
-  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
-    acc += lens[i] >= 0 ? lens[i] : (1ll << 40);  // a negative length is a row that itself passed 2^31
-  for (int o = 16; o; o >>= 1) acc += __shfl_down_sync(0xffffffffu, acc, o);
-  if ((threadIdx.x & 31) == 0) atomicAdd(total, (unsigned long long)acc);
-}
-
-}  // namespace
-
-// The offsets of a Binary / Utf8 column are int32, and so is pb_scan: when lengths add up to 2^31 or more the scan wraps,
-// and once it wraps past 2^32 its last entry looks valid again while earlier offsets point outside the allocation.  When
-// the host's bound on the total (`bound`) does not rule that out, the total is summed exactly first (one more launch and
-// synchronisation, taken only by batches near the limit) and a total beyond the int32 range fails before anything is
-// written.
-void pb_check_total(const int32_t* lens, int64_t n, int64_t bound, const std::string& what, cudaStream_t stream) {
-  if (bound >= 0 && bound <= INT32_MAX) return;
-  BufferPtr d = device_alloc(8), h = pinned_alloc(8);
-  ARK_CUDA(cudaMemsetAsync(d.get(), 0, 8, stream));
-  if (n > 0) {
-    KernelTimer t("protobuf_sum64_kernel", stream);
-    protobuf_sum64_kernel<<<(unsigned)std::min<int64_t>(ceil_div(n, 256), 8 * sm_count()), 256, 0, stream>>>(lens, n, (unsigned long long*)d.get());
-  }
-  ARK_CUDA(cudaMemcpyAsync(h.get(), d.get(), 8, cudaMemcpyDeviceToHost, stream));
-  ARK_CUDA(cudaStreamSynchronize(stream));
-  const unsigned long long total = *(const unsigned long long*)h.get();
-  if (total > (unsigned long long)INT32_MAX) fail(ARK_ERR_PROCESS, what + " holds " + std::to_string(total) + " bytes: more than a Binary / Utf8 column's 2 GiB");
-}
-
-// exclusive scan of n + 1 int32 lengths (pb_check_total guards the int32 range)
-BufferPtr pb_scan(const int32_t* lens, int64_t n, cudaStream_t stream) {
-  BufferPtr offs = device_alloc((size_t)(n + 1) * 4);
-  size_t tb = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, tb, lens, (int32_t*)offs.get(), (int)(n + 1), stream);
-  BufferPtr tmp = device_alloc(tb + 16);
-  note_launch("cub::DeviceScan::ExclusiveSum");
-  cub::DeviceScan::ExclusiveSum(tmp.get(), tb, lens, (int32_t*)offs.get(), (int)(n + 1), stream);
-  return offs;
-}
-
-// string / bytes column bytes from spans of `data`: row r = data[src[r] .. src[r] + offsets[r+1] - offsets[r])
-void launch_span_copy(const uint8_t* data, const long long* src, const int32_t* offsets, int64_t n_rows, uint8_t* out, cudaStream_t stream) {
-  if (n_rows == 0) return;
-  KernelTimer t("protobuf_strings_kernel", stream);
-  protobuf_strings_kernel<<<(unsigned)ceil_div(n_rows, 256), 256, 0, stream>>>(data, nullptr, src, offsets, n_rows, out);
-}
-
-namespace {
 
 // ---- configuration ----------------------------------------------------------------------------------------------
 std::vector<std::string> string_list(const JsonValue& v, const char* key) {
@@ -538,7 +474,7 @@ Batch protobuf_to_arrow_device(const Processor& proc, Batch& in, cudaStream_t st
       KernelTimer t("protobuf_valid_kernel", stream);
       protobuf_valid_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, stream>>>(col.validity, col.validity_bit0, n, (int32_t*)flags.get());
     }
-    row_of = pb_scan((const int32_t*)flags.get(), n, stream);
+    row_of = varlen_scan((const int32_t*)flags.get(), n, stream);
     ARK_CUDA(cudaMemcpyAsync(h.get(), (int32_t*)row_of.get() + n, 4, cudaMemcpyDeviceToHost, stream));
     ARK_CUDA(cudaStreamSynchronize(stream));
     rows = *(const int32_t*)h.get();
@@ -596,7 +532,7 @@ Batch protobuf_to_arrow_device(const Processor& proc, Batch& in, cudaStream_t st
   ARK_CUDA(cudaMemcpyAsync(h.get(), err.get(), 8, cudaMemcpyDeviceToHost, stream));
   for (size_t k = 0; k < nf; ++k) {
     if (!lens[k]) continue;
-    str_offs[k] = pb_scan((const int32_t*)lens[k].get(), rows, stream);
+    str_offs[k] = varlen_scan((const int32_t*)lens[k].get(), rows, stream);
     ARK_CUDA(cudaMemcpyAsync((char*)h.get() + 16 + 4 * k, (int32_t*)str_offs[k].get() + rows, 4, cudaMemcpyDeviceToHost, stream));
   }
   ARK_CUDA(cudaStreamSynchronize(stream));
@@ -606,7 +542,7 @@ Batch protobuf_to_arrow_device(const Processor& proc, Batch& in, cudaStream_t st
   // a row's span lies inside its own payload, so the payload bytes plus one default per row bound a string column's total
   for (size_t k = 0; k < nf; ++k)
     if (lens[k])
-      pb_check_total((const int32_t*)lens[k].get(), rows, col.data_bytes + rows * (int64_t)fields[k].default_bytes.size(),
+      varlen_guard((const int32_t*)lens[k].get(), rows, col.data_bytes + rows * (int64_t)fields[k].default_bytes.size(),
                      "protobuf_to_arrow: column '" + fields[k].name + "'", stream);
 
   // ---- columns ----
@@ -620,13 +556,8 @@ Batch protobuf_to_arrow_device(const Processor& proc, Batch& in, cudaStream_t st
     if (str_offs[k]) {
       const int32_t total = *(const int32_t*)((char*)h.get() + 16 + 4 * k);
       BufferPtr bytes = device_alloc((size_t)total + 16);
-      if (rows && total) {
-        KernelTimer tm("protobuf_strings_kernel", stream);
-        protobuf_strings_kernel<<<(unsigned)ceil_div(rows, 256), 256, 0, stream>>>(col.data, (const uint8_t*)blob.get(), (const long long*)src[k].get(),
-                                                                                 (const int32_t*)str_offs[k].get(), rows, (uint8_t*)bytes.get());
-      }
-      c.offsets = (const int32_t*)str_offs[k].get(); c.data = (const uint8_t*)bytes.get(); c.data_bytes = total; c.first_offset = 0;
-      c.owners = {str_offs[k], bytes};
+      if (total) launch_span_copy(col.data, (const uint8_t*)blob.get(), (const long long*)src[k].get(), (const int32_t*)str_offs[k].get(), rows, (uint8_t*)bytes.get(), stream);
+      set_varlen(c, {str_offs[k], bytes, total});
     } else if (t == DType::Bool) {
       BufferPtr bits = device_alloc((size_t)(rows + 7) / 8 + 1);
       if (rows) launch_pack_bits((const uint8_t*)values[k].get(), rows, (uint8_t*)bits.get(), nullptr, stream);
@@ -697,18 +628,11 @@ Batch arrow_to_protobuf_device(const Processor& proc, Batch& in, cudaStream_t st
     KernelTimer t("protobuf_encode_measure_kernel", stream);
     protobuf_encode_measure_kernel<<<grid, PB_THREADS, 0, stream>>>(P, (int32_t*)lens.get());
   }
-  pb_check_total((const int32_t*)lens.get(), n, bound, "arrow_to_protobuf: the encoded messages", stream);
-  BufferPtr offs = pb_scan((const int32_t*)lens.get(), n, stream);
-  BufferPtr h = pinned_alloc(16);
-  ARK_CUDA(cudaMemcpyAsync(h.get(), (int32_t*)offs.get() + n, 4, cudaMemcpyDeviceToHost, stream));
-  ARK_CUDA(cudaStreamSynchronize(stream));
-  const int32_t total = *(const int32_t*)h.get();
-  BufferPtr bytes = device_alloc((size_t)total + 16);
-  if (n && total) {
+  const Varlen out_v = varlen_layout((const int32_t*)lens.get(), n, nullptr, bound, "arrow_to_protobuf: the encoded messages", stream);
+  if (n && out_v.total) {
     KernelTimer t("protobuf_encode_write_kernel", stream);
-    // staging window: the average CTA's bytes + 50 %; CTAs whose rows are longer take the direct path
-    const int stage = (int)std::min<int64_t>(44 * 1024, round_up((int64_t)((double)total / (double)n * PB_THREADS * 1.5) + 256, 1024));
-    protobuf_encode_write_kernel<<<grid, PB_THREADS, stage, stream>>>(P, (const int32_t*)offs.get(), (uint8_t*)bytes.get(), stage);
+    const int stage = stage_window(out_v.total, n, PB_THREADS);
+    protobuf_encode_write_kernel<<<grid, PB_THREADS, stage, stream>>>(P, (const int32_t*)out_v.offsets.get(), (uint8_t*)out_v.bytes.get(), stage);
   }
   ARK_CUDA(cudaGetLastError());
   Batch out;
@@ -717,8 +641,7 @@ Batch arrow_to_protobuf_device(const Processor& proc, Batch& in, cudaStream_t st
   Column v;
   v.field.name = "__value__"; v.field.type = DType::Binary; v.field.nullable = false; v.field.format = "z";
   v.length = n;
-  v.offsets = (const int32_t*)offs.get(); v.data = (const uint8_t*)bytes.get(); v.data_bytes = total; v.first_offset = 0;
-  v.owners = {offs, bytes};
+  set_varlen(v, out_v);
   out.cols.push_back(v);
   ARK_CUDA(cudaStreamSynchronize(stream));
   return out;

@@ -2,7 +2,10 @@
 // destination-aligned 16-byte stores.  The staging buffer must start at the destination's misalignment
 // (stage_misalignment) so that shared and global addresses agree mod 16.
 #pragma once
+#include <algorithm>
 #include <cstdint>
+
+#include "common.h"
 
 namespace ark {
 
@@ -19,6 +22,12 @@ __device__ __forceinline__ void stage_store(uint8_t* gdst, const uint8_t* stage,
   for (int g = tid; g < body; g += nthreads) gv[g] = sv[g];
   const int tail0 = head + body * 16;
   if (tid < bytes - tail0) gdst[tail0 + tid] = stage[mis + tail0 + tid];
+}
+
+// Staging window of a kernel whose CTAs write `rows_per_cta` rows of a `total`-byte, `n`-row output through stage_store:
+// the average CTA's bytes + 50 %, at most 44 KiB.  CTAs whose rows are longer take the kernel's direct path.
+inline int stage_window(int64_t total, int64_t n, int rows_per_cta) {
+  return (int)std::min<int64_t>(44 * 1024, round_up((int64_t)((double)total / (double)n * rows_per_cta * 1.5) + 256, 1024));
 }
 
 }  // namespace ark

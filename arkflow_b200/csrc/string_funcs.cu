@@ -5,11 +5,10 @@
 // expr/mod.rs:148-166 — and from any SELECT list, processor/sql.rs:188-204).  NULL arguments count as
 // empty strings and the result is never NULL.  Runs after the row kernels on the surviving rows:
 // lengths → exclusive scan → one thread per row writes its parts.
-#include <cub/device/device_scan.cuh>
-
 #include "agg_acc.cuh"
 #include "engine.h"
 #include "stage_store.cuh"
+#include "varlen.h"
 
 namespace ark {
 
@@ -113,34 +112,24 @@ __global__ void __launch_bounds__(CONCAT_THREADS) concat_write_kernel(const __gr
 
 }  // namespace
 
-// lengths → scan → bytes for one string column described by P; returns the offsets / bytes of the n_rows strings
-static void render_strings(const ConcatParams& P, int64_t n, cudaStream_t stream, BufferPtr* out_offs, BufferPtr* out_bytes, int32_t* out_total) {
+// lengths → scan → bytes for one string column described by P: the offsets / bytes of the n_rows strings
+static Varlen render_strings(const ConcatParams& P, int64_t n, cudaStream_t stream) {
   // lens[n] = 0 closes the scan; the 64-bit total sits in the 8 bytes after it
-  BufferPtr lens = device_alloc((size_t)(n + 1) * 4 + 16), offs = device_alloc((size_t)(n + 1) * 4);
+  BufferPtr lens = device_alloc((size_t)(n + 1) * 4 + 16);
   const int64_t sum_at = round_up((int64_t)(n + 1) * 4, 8);
   ARK_CUDA(cudaMemsetAsync((int32_t*)lens.get() + n, 0, (size_t)(sum_at + 8 - n * 4), stream));
   unsigned long long* sum = (unsigned long long*)((uint8_t*)lens.get() + sum_at);
   const unsigned grid = (unsigned)std::max<int64_t>(1, ceil_div(n, 256));
   if (n) { KernelTimer t("concat_lengths_kernel", stream); concat_lengths_kernel<<<grid, 256, 0, stream>>>(P, (int32_t*)lens.get(), sum); }
-  size_t tb = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, tb, (int32_t*)lens.get(), (int32_t*)offs.get(), (int)(n + 1), stream);
-  BufferPtr tmp = device_alloc(tb + 16);
-  note_launch("cub::DeviceScan::ExclusiveSum");
-  cub::DeviceScan::ExclusiveSum(tmp.get(), tb, (int32_t*)lens.get(), (int32_t*)offs.get(), (int)(n + 1), stream);
-  BufferPtr h = pinned_alloc(64);
-  ARK_CUDA(cudaMemcpyAsync(h.get(), sum, 8, cudaMemcpyDeviceToHost, stream));
-  ARK_CUDA(cudaStreamSynchronize(stream));
-  const unsigned long long total64 = *(const unsigned long long*)h.get();
-  if (total64 > 2147483647ull) fail(ARK_ERR_PROCESS, "Collection query results error: Arrow error: offset overflow, string result exceeds 2 GiB");
-  const int32_t total = (int32_t)total64;  // = offs[n]: the scan did not wrap
-  BufferPtr bytes = device_alloc((size_t)total + 16);
+  Varlen v = varlen_layout((const int32_t*)lens.get(), n, sum, -1, "Collection query results error: Arrow error: offset overflow, string result exceeds 2 GiB",
+                           stream);
   if (n) {
-    const int stage = (int)std::min<int64_t>(44 * 1024, round_up((int64_t)((double)total / (double)n * CONCAT_THREADS * 1.5) + 256, 1024));
+    const int stage = stage_window(v.total, n, CONCAT_THREADS);
     KernelTimer t("concat_write_kernel", stream);
-    concat_write_kernel<<<grid, CONCAT_THREADS, stage, stream>>>(P, (const int32_t*)offs.get(), (uint8_t*)bytes.get(), stage);
+    concat_write_kernel<<<grid, CONCAT_THREADS, stage, stream>>>(P, (const int32_t*)v.offsets.get(), (uint8_t*)v.bytes.get(), stage);
   }
   ARK_CUDA(cudaGetLastError());
-  *out_offs = offs; *out_bytes = bytes; *out_total = total;
+  return v;
 }
 
 // CAST(<Int64 column> AS STRING) of an already materialised column (aggregate results): decimal text, NULL stays NULL
@@ -149,14 +138,10 @@ Column format_int64_column(const Column& src, const std::string& name, cudaStrea
   memset(&P, 0, sizeof P);
   P.n_parts = 1; P.n_rows = src.length;
   P.parts[0].data = src.data; P.parts[0].validity = src.validity; P.parts[0].validity_bit0 = (int32_t)src.validity_bit0; P.parts[0].kind = PART_INT64;
-  BufferPtr offs, bytes;
-  int32_t total = 0;
-  render_strings(P, src.length, stream, &offs, &bytes, &total);
   Column c;
   c.field.name = name; c.field.type = DType::Utf8; c.field.nullable = src.field.nullable; c.length = src.length;
-  c.offsets = (const int32_t*)offs.get(); c.data = (const uint8_t*)bytes.get(); c.data_bytes = total; c.first_offset = 0;
+  set_varlen(c, render_strings(P, src.length, stream));
   c.validity = src.validity; c.validity_bit0 = src.validity_bit0; c.null_count = src.null_count;
-  c.owners = {offs, bytes};
   for (auto& o : src.owners) c.owners.push_back(o);
   return c;
 }
@@ -193,15 +178,11 @@ Batch apply_concats(const Plan& plan, Batch& r, cudaStream_t stream) {
       }
     }
     if (lit_bytes) ARK_CUDA(cudaMemcpyAsync(lit_dev.get(), lit_host.get(), lit_bytes, cudaMemcpyHostToDevice, stream));
-    BufferPtr offs, bytes;
-    int32_t total = 0;
-    render_strings(P, n, stream, &offs, &bytes, &total);
-    ARK_CUDA(cudaStreamSynchronize(stream));  // the literal staging blocks go back to the pool
     Column& c = made[ci];
+    set_varlen(c, render_strings(P, n, stream));
+    ARK_CUDA(cudaStreamSynchronize(stream));  // the literal staging blocks go back to the pool
     c.field.name = item.name; c.field.type = DType::Utf8; c.field.nullable = true; c.length = n;
-    c.offsets = (const int32_t*)offs.get(); c.data = (const uint8_t*)bytes.get(); c.data_bytes = total; c.first_offset = 0;
     c.validity = nullptr; c.null_count = 0;
-    c.owners = {offs, bytes};
     if (item.is_cast && !item.parts.empty() && !item.parts[0].is_literal) {  // CAST: NULL in ⇒ NULL out — the source's bitmap is the result's
       const Column& src = r.cols[item.parts[0].out_index];
       c.field.nullable = src.field.nullable;
