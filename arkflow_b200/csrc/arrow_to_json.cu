@@ -12,6 +12,7 @@
 // Two passes, one thread per row: measure → exclusive scan → write.
 #include <algorithm>
 
+#include "bitmap.cuh"
 #include "engine.h"
 #include "stage_store.cuh"
 #include "json_mini.h"
@@ -248,7 +249,7 @@ __device__ unsigned emit_row(const AjParams& P, int64_t row, uint8_t* out) {
     const AjCol& col = P.cols[c];
     if ((DType)col.dtype == DType::Null) continue;
     const ColView& v = col.view;
-    if (v.validity && !((v.validity[(row + v.validity_bit0) >> 3] >> ((row + v.validity_bit0) & 7)) & 1)) continue;
+    if (!col_valid(v, row)) continue;
     if (!first) s.put(',');
     first = false;
     for (int i = 0; i < col.key_len; ++i) s.put((uint8_t)col.key[i]);
@@ -256,8 +257,7 @@ __device__ unsigned emit_row(const AjParams& P, int64_t row, uint8_t* out) {
       case DType::Int64: put_i64(s, ((const long long*)v.data)[row]); break;
       case DType::Float64: put_f64(s, ((const unsigned long long*)v.data)[row]); break;
       case DType::Bool: {
-        const int64_t b = row + v.data_bit0;
-        const bool t = (((const uint8_t*)v.data)[b >> 3] >> (b & 7)) & 1;
+        const bool t = bit_get((const uint8_t*)v.data, row + v.data_bit0);
         const char* w = t ? "true" : "false";
         for (int i = 0; w[i]; ++i) s.put((uint8_t)w[i]);
         break;

@@ -32,6 +32,7 @@
 #include <algorithm>
 #include <cstdio>
 
+#include "bitmap.h"
 #include "engine.h"
 #include "json_mini.h"
 #include "tma.cuh"
@@ -696,7 +697,7 @@ Batch avro_batch(AvroFile& f, const BufferPtr& file_dev, int64_t r0, int64_t n, 
       if (lens[k]) varlen_guard((const int32_t*)lens[k].get(), n, bound, "avro input: column '" + f.fields[k].name + "'", stream);
   }
   // the error word, every string total and every null count come back in one round trip
-  std::vector<BufferPtr> offs(nf), vbits(nf), bits(nf);
+  std::vector<BufferPtr> offs(nf), vbits(nf);
   BufferPtr zeros = device_alloc(8 * std::max<size_t>(nf, 1));
   ARK_CUDA(cudaMemsetAsync(zeros.get(), 0, 8 * std::max<size_t>(nf, 1), stream));
   ARK_CUDA(cudaMemcpyAsync(h.get(), err.get(), 8, cudaMemcpyDeviceToHost, stream));
@@ -706,8 +707,7 @@ Batch avro_batch(AvroFile& f, const BufferPtr& file_dev, int64_t r0, int64_t n, 
       ARK_CUDA(cudaMemcpyAsync((char*)h.get() + 8 + 16 * k, (int32_t*)offs[k].get() + n, 4, cudaMemcpyDeviceToHost, stream));
     }
     if (valid[k]) {
-      vbits[k] = device_alloc((size_t)(n + 7) / 8 + 1);
-      launch_pack_bits((const uint8_t*)valid[k].get(), n, (uint8_t*)vbits[k].get(), (unsigned long long*)zeros.get() + k, stream);
+      vbits[k] = pack_bits((const uint8_t*)valid[k].get(), n, (unsigned long long*)zeros.get() + k, stream);
       ARK_CUDA(cudaMemcpyAsync((char*)h.get() + 16 + 16 * k, (unsigned long long*)zeros.get() + k, 8, cudaMemcpyDeviceToHost, stream));
     }
   }
@@ -730,14 +730,11 @@ Batch avro_batch(AvroFile& f, const BufferPtr& file_dev, int64_t r0, int64_t n, 
       if (total) launch_span_copy(P.arena, nullptr, (const long long*)src[k].get(), (const int32_t*)offs[k].get(), n, (uint8_t*)bytes.get(), stream);
       set_varlen(c, {offs[k], bytes, total});
     } else if (t == DType::Bool) {
-      BufferPtr bb = device_alloc((size_t)(n + 7) / 8 + 1);
-      launch_pack_bits((const uint8_t*)values[k].get(), n, (uint8_t*)bb.get(), nullptr, stream);
-      c.data = (const uint8_t*)bb.get(); c.data_bytes = (n + 7) / 8; c.owners = {bb};
+      set_bool_values(c, values[k], n, stream);
     } else {
       c.data = (const uint8_t*)values[k].get(); c.data_bytes = n * fixed_width(t); c.owners = {values[k]};
     }
-    const long long nulls = valid[k] ? *(const long long*)((char*)h.get() + 16 + 16 * k) : 0;
-    if (nulls > 0) { c.validity = (const uint8_t*)vbits[k].get(); c.validity_bit0 = 0; c.null_count = nulls; c.owners.push_back(vbits[k]); }
+    set_validity(c, vbits[k], valid[k] ? *(const long long*)((char*)h.get() + 16 + 16 * k) : 0);
     out.cols.push_back(std::move(c));
   }
   ARK_CUDA(cudaGetLastError());

@@ -9,6 +9,7 @@
 #include <thread>
 
 #include "batch.h"
+#include "bitmap.h"
 
 namespace ark {
 
@@ -799,20 +800,6 @@ __global__ void rebase_offsets_kernel(const int32_t* in, int32_t* out, int64_t n
   int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n1) out[i] = in[i] - first;
 }
-// copy `n` bits starting at bit `bit0` of `in` into a fresh bitmap starting at bit 0
-__global__ void realign_bits_kernel(const uint8_t* in, uint8_t* out, int64_t n, int32_t bit0) {
-  int64_t byte = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  int64_t nbytes = (n + 7) >> 3;
-  if (byte >= nbytes) return;
-  int64_t src_bit = byte * 8 + bit0;
-  uint32_t lo = in[src_bit >> 3];
-  uint32_t hi = (((src_bit & 7) != 0) && ((src_bit >> 3) + 1 <= ((bit0 + n - 1) >> 3))) ? in[(src_bit >> 3) + 1] : 0;
-  uint32_t v = ((lo | (hi << 8)) >> (src_bit & 7)) & 0xff;
-  int64_t rem = n - byte * 8;
-  if (rem < 8) v &= (1u << rem) - 1;
-  out[byte] = (uint8_t)v;
-}
-
 }  // namespace
 
 static void fill_column_schema(ArrowSchema* s, const Column& c) {
@@ -871,9 +858,7 @@ static ExportCol normalise_for_export(const Column& c_in, bool to_host, cudaStre
   if (c.validity && c.null_count != 0 && n > 0) {
     e.validity_bytes = (n + 7) / 8;
     if (c.validity_bit0 != 0) {
-      BufferPtr v = device_alloc((size_t)e.validity_bytes);
-      KernelTimer t("realign_bits_kernel", stream);
-      realign_bits_kernel<<<(unsigned)ceil_div(e.validity_bytes, 256), 256, 0, stream>>>(c.validity, (uint8_t*)v.get(), n, c.validity_bit0);
+      BufferPtr v = realign_bits(c.validity, c.validity_bit0, n, stream);
       e.validity = (const uint8_t*)v.get(); e.owners.push_back(v);
     } else e.validity = c.validity;
   }
@@ -884,9 +869,7 @@ static ExportCol normalise_for_export(const Column& c_in, bool to_host, cudaStre
     case DType::Bool:
       e.buf1_bytes = (n + 7) / 8;
       if (c.data_bit0 != 0 && n > 0) {
-        BufferPtr v = device_alloc((size_t)e.buf1_bytes);
-        KernelTimer t("realign_bits_kernel", stream);
-        realign_bits_kernel<<<(unsigned)ceil_div(e.buf1_bytes, 256), 256, 0, stream>>>(c.data, (uint8_t*)v.get(), n, c.data_bit0);
+        BufferPtr v = realign_bits(c.data, c.data_bit0, n, stream);
         e.buf1 = v.get(); e.owners.push_back(v);
       } else e.buf1 = c.data;
       e.n_buffers = 2; break;

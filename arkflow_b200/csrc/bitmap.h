@@ -1,0 +1,40 @@
+// bitmap.h — the Arrow bitmaps (validity and Boolean values) the library builds on the device from one byte per row,
+// and the null count that goes with a validity bitmap.  bitmap.cuh reads them on the device.
+//
+// A bitmap of n rows starts at bit 0, and the unused bits of its last byte are zero.  It is allocated with
+// (n + 7) / 8 + 1 bytes, of which the first (n + 7) / 8 are the bitmap.
+//
+// A column's null_count is exact or -1 (unknown), and a column whose count is 0 carries no validity bitmap.  Which of
+// the two a producer gives depends on what the count costs it:
+//   * exact: the inputs and decoders (CSV, JSON, Avro) count the zero bytes while packing and read the count back.
+//     A single-column producer does it in set_validity_exact, one synchronisation per column.  A producer that makes one
+//     round trip for all its columns' totals gives pack_bits a counter slot of that round trip and calls set_validity
+//     after its synchronisation.
+//   * unknown: query outputs (SQL projection, join gathers, GROUP BY keys and aggregates) take no read-back and no
+//     synchronisation; set_validity_unknown attaches the bitmap whenever there are rows.
+#pragma once
+#include "batch.h"
+
+namespace ark {
+
+// bytes[0 .. n) (0 / non-zero) packed into a fresh bitmap.  `zeros` (may be null): a device counter the number of zero
+// bytes is added to.
+BufferPtr pack_bits(const uint8_t* bytes, int64_t n, unsigned long long* zeros, cudaStream_t stream);
+
+// c.data / data_bit0 / data_bytes: bytes[0 .. n) packed; owners = {bitmap, bytes}: validity owners go after.
+void set_bool_values(Column& c, const BufferPtr& bytes, int64_t n, cudaStream_t stream);
+
+// Attaches `bits` as c's validity with `null_count` (-1: unknown); a count of 0 attaches nothing.
+void set_validity(Column& c, const BufferPtr& bits, int64_t null_count);
+
+// c's validity from bytes[0 .. n) with its exact null count: one read-back and one synchronisation when n > 0.  `bytes`
+// is not kept.
+void set_validity_exact(Column& c, const uint8_t* bytes, int64_t n, cudaStream_t stream);
+
+// c's validity from bytes[0 .. n) with null_count -1, attached when n > 0 and kept alive with `bytes`.
+void set_validity_unknown(Column& c, const BufferPtr& bytes, int64_t n, cudaStream_t stream);
+
+// The n bits of `in` from bit `bit0` on, copied into a fresh bitmap of (n + 7) / 8 bytes that starts at bit 0.  n > 0.
+BufferPtr realign_bits(const uint8_t* in, int32_t bit0, int64_t n, cudaStream_t stream);
+
+}  // namespace ark

@@ -7,6 +7,7 @@
 // (SURVEY.md §8(d) config 5: 2 × 32 B/row for decoded S, 134 B/msg for raw Binary payloads).
 #include <algorithm>
 
+#include "bitmap.cuh"
 #include "engine.h"
 
 namespace ark {
@@ -115,7 +116,7 @@ __global__ void concat_bits_kernel(const BitSeg* segs, int n_segs, long long tot
     while (seg + 1 < n_segs && segs[seg + 1].row0 <= r) ++seg;
     const BitSeg s = segs[seg];
     const long long p = r - s.row0 + s.bit0;
-    const unsigned bit = s.bits ? (s.bits[p >> 3] >> (p & 7)) & 1u : 1u;
+    const unsigned bit = s.bits ? bit_get(s.bits, p) : 1u;
     v |= bit << i;
   }
   out[ob] = (uint8_t)v;

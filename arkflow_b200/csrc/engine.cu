@@ -3,6 +3,7 @@
 
 #include <algorithm>
 
+#include "bitmap.h"
 #include "json_mini.h"
 
 namespace ark {
@@ -402,19 +403,12 @@ Batch run_filter_project(const Plan& plan, Batch& in, cudaStream_t stream) {
           c.data_bytes = totals[1 + vseen]; c.first_offset = 0; ++vseen;
           c.owners = {po.offsets, po.data};
         } else if (po.is_bool) {
-          BufferPtr bits = device_alloc((size_t)(count + 7) / 8 + 1);
-          launch_pack_bits((const uint8_t*)po.data.get(), count, (uint8_t*)bits.get(), nullptr, stream);
-          c.data = (const uint8_t*)bits.get(); c.data_bit0 = 0; c.data_bytes = (count + 7) / 8;
-          c.owners = {bits, po.data};
+          set_bool_values(c, po.data, count, stream);
         } else {
           c.data = (const uint8_t*)po.data.get(); c.data_bytes = count * 8; c.owners = {po.data};
         }
-        if (po.valid_bytes && count > 0) {
-          BufferPtr bits = device_alloc((size_t)(count + 7) / 8 + 1);
-          launch_pack_bits((const uint8_t*)po.valid_bytes.get(), count, (uint8_t*)bits.get(), nullptr, stream);
-          c.validity = (const uint8_t*)bits.get(); c.validity_bit0 = 0; c.null_count = -1;
-          c.owners.push_back(bits); c.owners.push_back(po.valid_bytes);
-        } else { c.validity = nullptr; c.null_count = 0; }
+        if (po.valid_bytes) set_validity_unknown(c, po.valid_bytes, count, stream);
+        else set_validity(c, nullptr, 0);
         (void)oc;
       }
     }

@@ -31,7 +31,6 @@ Column format_int64_column(const Column& src, const std::string& name, cudaStrea
 void launch_filter_project(const FpParams& P, int pred_kind, cudaStream_t stream);
 void launch_utf8_validate(const int32_t* offsets, const uint8_t* data, const uint8_t* validity, int vbit0, int64_t n, int* bad, cudaStream_t stream);
 const char* vm_error_text(int vm_error);  // arrow-arith / arrow-cast message of a VmError
-void launch_pack_bits(const uint8_t* bytes, int64_t n, uint8_t* bitmap, unsigned long long* zeros, cudaStream_t stream);
 
 struct Processor {
   virtual ~Processor() {}

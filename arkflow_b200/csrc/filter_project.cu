@@ -331,28 +331,11 @@ __global__ void __launch_bounds__(FP_THREADS) filter_project_kernel(const __grid
   if (err) atomicExch(P.error, err);
 }
 
-// byte-per-row (0/1) → bitmap; counts zero bytes into *zeros (null count for validity maps)
-__global__ void pack_bits_kernel(const uint8_t* bytes, int64_t n, uint8_t* bitmap, unsigned long long* zeros) {
-  int64_t ob = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  int64_t nb = (n + 7) >> 3;
-  int z = 0;
-  if (ob < nb) {
-    unsigned v = 0;
-    for (int i = 0; i < 8; ++i) {
-      int64_t r = ob * 8 + i;
-      if (r < n) { if (bytes[r]) v |= 1u << i; else ++z; }
-    }
-    bitmap[ob] = (uint8_t)v;
-  }
-  z = (int)warp_sum(z);
-  if ((threadIdx.x & 31) == 0 && z && zeros) atomicAdd(zeros, (unsigned long long)z);
-}
-
 // One thread validates one string (utf8_valid).  Raises *bad when any non-NULL string is invalid.
 __global__ void utf8_validate_kernel(const int32_t* offsets, const uint8_t* data, const uint8_t* validity, int vbit0, long long n, int* bad) {
   const long long r = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= n) return;
-  if (validity && !((validity[(r + vbit0) >> 3] >> ((r + vbit0) & 7)) & 1)) return;
+  if (validity && !bit_get(validity, r + vbit0)) return;
   if (!utf8_valid(data + offsets[r], offsets[r + 1] - offsets[r])) atomicExch(bad, 1);
 }
 
@@ -378,13 +361,6 @@ void launch_utf8_validate(const int32_t* offsets, const uint8_t* data, const uin
   if (n <= 0) return;
   KernelTimer t("utf8_validate_kernel", stream);
   utf8_validate_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, stream>>>(offsets, data, validity, vbit0, n, bad);
-}
-
-void launch_pack_bits(const uint8_t* bytes, int64_t n, uint8_t* bitmap, unsigned long long* zeros, cudaStream_t stream) {
-  if (n <= 0) return;
-  KernelTimer t("pack_bits_kernel", stream);
-  int64_t nb = (n + 7) >> 3;
-  pack_bits_kernel<<<(unsigned)ceil_div(nb, 256), 256, 0, stream>>>(bytes, n, bitmap, zeros);
 }
 
 }  // namespace ark

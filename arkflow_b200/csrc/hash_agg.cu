@@ -11,6 +11,7 @@
 // Algorithmic traffic = key + argument bytes read once (SURVEY.md §8(d): 24 B/row for config 3).
 
 #include "agg_acc.cuh"
+#include "bitmap.h"
 #include "engine.h"
 #include "group_exchange.h"
 #include "hash_agg.cuh"
@@ -563,21 +564,15 @@ static Column emit_key_column(const AggExec& ex, const DenseGroups& dg, const Co
     }
     c.data = (const uint8_t*)vals.get(); c.data_bytes = (int64_t)G * 8; c.owners = {vals};
   } else {  // KEY_BOOL
-    BufferPtr bb = device_alloc(std::max<size_t>(G, 1)), bits = device_alloc((size_t)(G + 7) / 8 + 1);
+    BufferPtr bb = device_alloc(std::max<size_t>(G, 1));
     if (G) {
       KernelTimer t("agg_emit_keys_kernel", stream);
       agg_emit_keys_kernel<<<grid, 256, 0, stream>>>(keys, kstride, slots, G, kc, ex.key_kind, nullptr, (uint8_t*)bb.get(), nullptr, nullptr,
                                                      (uint8_t*)valid_bytes.get());
     }
-    launch_pack_bits((const uint8_t*)bb.get(), G, (uint8_t*)bits.get(), nullptr, stream);
-    c.data = (const uint8_t*)bits.get(); c.data_bytes = (G + 7) / 8; c.owners = {bits, bb};
+    set_bool_values(c, bb, G, stream);
   }
-  if (may_null && G) {
-    BufferPtr vbits = device_alloc((size_t)(G + 7) / 8 + 1);
-    launch_pack_bits((const uint8_t*)valid_bytes.get(), G, (uint8_t*)vbits.get(), nullptr, stream);
-    c.validity = (const uint8_t*)vbits.get(); c.null_count = -1;
-    c.owners.push_back(vbits); c.owners.push_back(valid_bytes);
-  }
+  if (may_null) set_validity_unknown(c, valid_bytes, G, stream);
   return c;
 }
 
@@ -626,12 +621,7 @@ static Column finalize_column(const std::string& name, DType type, int op, Buffe
                                                                        constant, G, (unsigned long long*)out.get(), (uint8_t*)vb.get());
   }
   c.data = (const uint8_t*)out.get(); c.data_bytes = (int64_t)G * 8; c.owners = {out};
-  if (vb && G) {
-    BufferPtr bits = device_alloc((size_t)(G + 7) / 8 + 1);
-    launch_pack_bits((const uint8_t*)vb.get(), G, (uint8_t*)bits.get(), nullptr, stream);
-    c.validity = (const uint8_t*)bits.get(); c.null_count = -1;
-    c.owners.push_back(bits); c.owners.push_back(vb);
-  }
+  if (vb) set_validity_unknown(c, vb, G, stream);
   return c;
 }
 

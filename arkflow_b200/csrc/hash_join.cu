@@ -14,6 +14,8 @@
 #include <cub/device/device_scan.cuh>
 
 #include "agg_acc.cuh"
+#include "bitmap.cuh"
+#include "bitmap.h"
 #include "engine.h"
 #include "hashkey.cuh"
 #include "stage_store.cuh"
@@ -113,7 +115,7 @@ __global__ void take_bits_kernel(const uint8_t* bits, int bit0, const unsigned i
   if (i < n) {
     const unsigned int r = idx[i];
     const long long p = (long long)r + bit0;
-    out_bytes[i] = r == NO_ROW ? 0 : ((bits[p >> 3] >> (p & 7)) & 1);  // NO_ROW (outer join, no match): NULL / false
+    out_bytes[i] = r == NO_ROW ? 0 : bit_get(bits, p);  // NO_ROW (outer join, no match): NULL / false
   }
 }
 // validity of a gathered column that had none: only the NO_ROW rows are NULL
@@ -325,10 +327,9 @@ Column take_column(const Column& src, const unsigned int* idx, int64_t n, const 
       break;
     }
     case DType::Bool: {
-      BufferPtr bytes = device_alloc((size_t)std::max<int64_t>(n, 1)), bits = device_alloc((size_t)(n + 7) / 8 + 1);
+      BufferPtr bytes = device_alloc((size_t)std::max<int64_t>(n, 1));
       if (n) { KernelTimer t("take_bits_kernel", stream); take_bits_kernel<<<g, 256, 0, stream>>>(src.data, src.data_bit0, idx, n, (uint8_t*)bytes.get()); }
-      launch_pack_bits((const uint8_t*)bytes.get(), n, (uint8_t*)bits.get(), nullptr, stream);
-      c.data = (const uint8_t*)bits.get(); c.data_bit0 = 0; c.data_bytes = (n + 7) / 8; c.owners = {bits, bytes};
+      set_bool_values(c, bytes, n, stream);
       break;
     }
     case DType::Utf8: case DType::Binary: {
@@ -352,13 +353,11 @@ Column take_column(const Column& src, const unsigned int* idx, int64_t n, const 
   }
   if (may_miss) c.field.nullable = true;
   if ((src.validity || may_miss) && n > 0) {
-    BufferPtr vb = device_alloc((size_t)n), bits = device_alloc((size_t)(n + 7) / 8 + 1);
+    BufferPtr vb = device_alloc((size_t)n);
     if (src.validity) { KernelTimer t("take_bits_kernel", stream); take_bits_kernel<<<g, 256, 0, stream>>>(src.validity, src.validity_bit0, idx, n, (uint8_t*)vb.get()); }
     else { KernelTimer t("take_matched_kernel", stream); take_matched_kernel<<<g, 256, 0, stream>>>(idx, n, (uint8_t*)vb.get()); }
-    launch_pack_bits((const uint8_t*)vb.get(), n, (uint8_t*)bits.get(), nullptr, stream);
-    c.validity = (const uint8_t*)bits.get(); c.validity_bit0 = 0; c.null_count = -1;
-    c.owners.push_back(bits); c.owners.push_back(vb);
-  } else { c.validity = nullptr; c.null_count = 0; }
+    set_validity_unknown(c, vb, n, stream);
+  }
   return c;
 }
 

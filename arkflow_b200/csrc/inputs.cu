@@ -45,6 +45,7 @@
 #include <thrust/count.h>
 #include <thrust/execution_policy.h>
 
+#include "bitmap.h"
 #include "decimal.cuh"
 #include "engine.h"
 #include "json_mini.h"
@@ -548,12 +549,7 @@ Batch csv_batch(ark_input* in, int64_t l0, int64_t n, cudaStream_t stream) {
     switch (in->csv_types[c]) {
       case CSV_I64: col.field.type = DType::Int64; col.field.format = "l"; col.data = (const uint8_t*)vals[c].get(); col.data_bytes = n * 8; col.owners = {vals[c]}; break;
       case CSV_F64: col.field.type = DType::Float64; col.field.format = "g"; col.data = (const uint8_t*)vals[c].get(); col.data_bytes = n * 8; col.owners = {vals[c]}; break;
-      case CSV_BOOL: {
-        BufferPtr bits = device_alloc((size_t)(n + 7) / 8 + 1);
-        launch_pack_bits((const uint8_t*)vals[c].get(), n, (uint8_t*)bits.get(), nullptr, stream);
-        col.field.type = DType::Bool; col.field.format = "b"; col.data = (const uint8_t*)bits.get(); col.data_bytes = (n + 7) / 8; col.owners = {bits, vals[c]};
-        break;
-      }
+      case CSV_BOOL: col.field.type = DType::Bool; col.field.format = "b"; set_bool_values(col, vals[c], n, stream); break;
       default: {
         // a field's bytes lie inside its line, so the batch's byte span (at most 2 GiB, checked above) bounds the column
         const Varlen v = varlen_layout((const int32_t*)slen[c].get(), n, nullptr, byte1 - byte0, "file input: column '" + in->csv_names[c] + "'", stream);
@@ -566,16 +562,7 @@ Batch csv_batch(ark_input* in, int64_t l0, int64_t n, cudaStream_t stream) {
         break;
       }
     }
-    BufferPtr vbits = device_alloc((size_t)(n + 7) / 8 + 1);
-    BufferPtr zeros = device_alloc(16);
-    ARK_CUDA(cudaMemsetAsync(zeros.get(), 0, 16, stream));
-    launch_pack_bits((const uint8_t*)valid[c].get(), n, (uint8_t*)vbits.get(), (unsigned long long*)zeros.get(), stream);
-    BufferPtr hz = pinned_alloc(16);
-    ARK_CUDA(cudaMemcpyAsync(hz.get(), zeros.get(), 8, cudaMemcpyDeviceToHost, stream));
-    ARK_CUDA(cudaStreamSynchronize(stream));
-    const long long nulls = *(long long*)hz.get();
-    if (nulls > 0) { col.validity = (const uint8_t*)vbits.get(); col.validity_bit0 = 0; col.null_count = nulls; col.owners.push_back(vbits); }
-    else { col.validity = nullptr; col.null_count = 0; }
+    set_validity_exact(col, (const uint8_t*)valid[c].get(), n, stream);
     b.cols.push_back(std::move(col));
   }
   return b;

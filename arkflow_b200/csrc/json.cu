@@ -18,6 +18,8 @@
 #include <algorithm>
 #include <cmath>
 
+#include "bitmap.cuh"
+#include "bitmap.h"
 #include "engine.h"
 #include "tma.cuh"
 #include "json_mini.h"
@@ -375,7 +377,7 @@ __global__ void __launch_bounds__(JS_THREADS, 9) json_parse_kernel(const __grid_
   const long long stage_off = staged ? s_stage_off : 0;
   if (staged) mbar_wait(&s_bar, 0);
   if (i >= P.n_payloads) return;
-  if (P.validity && !((P.validity[(i + P.validity_bit0) >> 3] >> ((i + P.validity_bit0) & 7)) & 1)) {
+  if (P.validity && !bit_get(P.validity, i + P.validity_bit0)) {
     if (MODE == 0) P.counts[i] = 0;
     if (MODE == 2) P.error[2] = 1;
     return;
@@ -764,7 +766,7 @@ const char* json_err_text(int code) {
 }
 
 // A scalar column (values / strings / validity) of `rows` rows being decoded.
-struct FieldBufs { BufferPtr values, valid_bytes, str_len, str_src, str_raw, str_offsets, vbits; };
+struct FieldBufs { BufferPtr values, valid_bytes, str_len, str_src, str_raw, str_offsets; };
 
 void alloc_field(DType type, int64_t rows, FieldBufs& fb, JsonField& F, cudaStream_t stream) {
   fb.valid_bytes = device_alloc((size_t)std::max<int64_t>(rows, 1));
@@ -788,10 +790,7 @@ Column finish_scalar(const std::string& name, DType type, int64_t rows, FieldBuf
   if (type == DType::Null) { c.field.format = "n"; return c; }
   BufferPtr nulls = device_alloc(16), h = pinned_alloc(32);
   ARK_CUDA(cudaMemsetAsync(nulls.get(), 0, 16, stream));
-  if (rows > 0) {
-    fb.vbits = device_alloc((size_t)(rows + 7) / 8 + 1);
-    launch_pack_bits((const uint8_t*)fb.valid_bytes.get(), rows, (uint8_t*)fb.vbits.get(), (unsigned long long*)nulls.get(), stream);
-  }
+  BufferPtr vbits = pack_bits((const uint8_t*)fb.valid_bytes.get(), rows, (unsigned long long*)nulls.get(), stream);
   ARK_CUDA(cudaMemcpyAsync(h.get(), nulls.get(), 8, cudaMemcpyDeviceToHost, stream));
   if (type == DType::Utf8) {
     // a decoded string is never longer than its raw span inside the input column
@@ -803,9 +802,7 @@ Column finish_scalar(const std::string& name, DType type, int64_t rows, FieldBuf
   if (type == DType::Int64 || type == DType::Float64) {
     c.data = (const uint8_t*)fb.values.get(); c.data_bytes = rows * 8; c.owners = {fb.values};
   } else if (type == DType::Bool) {
-    BufferPtr bits = device_alloc((size_t)(rows + 7) / 8 + 1);
-    launch_pack_bits((const uint8_t*)fb.values.get(), rows, (uint8_t*)bits.get(), nullptr, stream);
-    c.data = (const uint8_t*)bits.get(); c.data_bytes = (rows + 7) / 8; c.owners = {bits, fb.values};
+    set_bool_values(c, fb.values, rows, stream);
   } else if (type == DType::Utf8) {
     const int32_t total = *(const int32_t*)((char*)h.get() + 8);
     BufferPtr bytes = device_alloc((size_t)total + 16);
@@ -816,8 +813,7 @@ Column finish_scalar(const std::string& name, DType type, int64_t rows, FieldBuf
     }
     set_varlen(c, {fb.str_offsets, bytes, total});
   }
-  const long long n_null = *(const long long*)h.get();
-  if (rows > 0 && n_null > 0) { c.validity = (const uint8_t*)fb.vbits.get(); c.null_count = n_null; c.owners.push_back(fb.vbits); }
+  set_validity(c, vbits, *(const long long*)h.get());
   return c;
 }
 
@@ -859,17 +855,7 @@ Column finish_list(const InferredField& f, int64_t rows, FieldBufs& fb, const ui
   Column child = finish_scalar("item", f.elem, total, cb, data, data_bytes, stream);  // arrow-rs names a list's field "item"
   Column c;
   c.field.name = f.name; c.field.type = DType::List; c.field.format = "+l"; c.field.nullable = true; c.length = rows;
-  // row validity
-  BufferPtr nulls = device_alloc(16), hn = pinned_alloc(16);
-  ARK_CUDA(cudaMemsetAsync(nulls.get(), 0, 16, stream));
-  if (rows > 0) {
-    BufferPtr vb = device_alloc((size_t)(rows + 7) / 8 + 1);
-    launch_pack_bits((const uint8_t*)fb.valid_bytes.get(), rows, (uint8_t*)vb.get(), (unsigned long long*)nulls.get(), stream);
-    ARK_CUDA(cudaMemcpyAsync(hn.get(), nulls.get(), 8, cudaMemcpyDeviceToHost, stream));
-    ARK_CUDA(cudaStreamSynchronize(stream));
-    const long long n_null = *(const long long*)hn.get();
-    if (n_null > 0) { c.validity = (const uint8_t*)vb.get(); c.null_count = n_null; c.owners.push_back(vb); }
-  }
+  set_validity_exact(c, (const uint8_t*)fb.valid_bytes.get(), rows, stream);
   c.offsets = (const int32_t*)offs.get(); c.first_offset = 0;
   c.owners.push_back(offs);
   c.children.push_back(std::move(child));
@@ -1023,16 +1009,7 @@ bool decode_fields(const std::vector<InferredField>& specs, JsonParams Q, unsign
       }
       Column c;
       c.field.name = f.name; c.field.type = DType::Struct; c.field.format = "+s"; c.field.nullable = true; c.length = rows;
-      BufferPtr nulls = device_alloc(16), hn = pinned_alloc(16);
-      ARK_CUDA(cudaMemsetAsync(nulls.get(), 0, 16, stream));
-      if (rows > 0) {
-        BufferPtr vb = device_alloc((size_t)(rows + 7) / 8 + 1);
-        launch_pack_bits((const uint8_t*)fb[k].valid_bytes.get(), rows, (uint8_t*)vb.get(), (unsigned long long*)nulls.get(), stream);
-        ARK_CUDA(cudaMemcpyAsync(hn.get(), nulls.get(), 8, cudaMemcpyDeviceToHost, stream));
-        ARK_CUDA(cudaStreamSynchronize(stream));
-        const long long n_null = *(const long long*)hn.get();
-        if (n_null > 0) { c.validity = (const uint8_t*)vb.get(); c.null_count = n_null; c.owners.push_back(vb); }
-      }
+      set_validity_exact(c, (const uint8_t*)fb[k].valid_bytes.get(), rows, stream);
       c.children = std::move(kids);
       out_cols.push_back(std::move(c));
     } else out_cols.push_back(finish_scalar(f.name, f.type, rows, fb[k], data, data_bytes, stream));

@@ -35,6 +35,8 @@
 // bytes column or an encoded message column of 2 GiB or more (int32 offsets) raises Process before anything is written.
 #include <algorithm>
 
+#include "bitmap.cuh"
+#include "bitmap.h"
 #include "engine.h"
 #include "json_mini.h"
 #include "proto_schema.h"
@@ -210,7 +212,7 @@ __global__ void __launch_bounds__(PB_THREADS) protobuf_decode_kernel(const __gri
   const bool staged = s_staged != 0;
   if (staged) mbar_wait(&s_bar, 0);
   if (i >= P.n_payloads) return;
-  if (P.validity && !((P.validity[(i + P.validity_bit0) >> 3] >> ((i + P.validity_bit0) & 7)) & 1)) return;
+  if (P.validity && !bit_get(P.validity, i + P.validity_bit0)) return;
   const int64_t row = P.row_of ? P.row_of[i] : i;
   // `origin` + column byte offset = address of that byte (in the staging window or in global memory)
   const uint8_t* origin = staged ? pb_stage - s_stage_off : P.data;
@@ -266,7 +268,7 @@ __global__ void __launch_bounds__(PB_THREADS) protobuf_decode_kernel(const __gri
 // 1 per non-NULL payload (the row count scan of a payload column with NULLs)
 __global__ void protobuf_valid_kernel(const uint8_t* validity, int32_t bit0, int64_t n, int32_t* flags) {
   const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) flags[i] = (validity[(i + bit0) >> 3] >> ((i + bit0) & 7)) & 1;
+  if (i < n) flags[i] = bit_get(validity, i + bit0);
 }
 
 // ---- encode -----------------------------------------------------------------------------------------------------
@@ -318,12 +320,7 @@ __device__ __forceinline__ long long pb_emit_row(const PbEncParams& P, int64_t r
     unsigned long long raw;
     bool zero;
     switch (k) {
-      case PbKind::Bool: {
-        const int64_t b = row + v.data_bit0;
-        raw = (((const uint8_t*)v.data)[b >> 3] >> (b & 7)) & 1;
-        zero = raw == 0;
-        break;
-      }
+      case PbKind::Bool: raw = bit_get((const uint8_t*)v.data, row + v.data_bit0); zero = raw == 0; break;
       case PbKind::Int32: case PbKind::SInt32: case PbKind::SFixed32: case PbKind::Enum:
       case PbKind::UInt32: case PbKind::Fixed32:
         raw = ((const uint32_t*)v.data)[row]; zero = raw == 0; break;
@@ -559,9 +556,7 @@ Batch protobuf_to_arrow_device(const Processor& proc, Batch& in, cudaStream_t st
       if (total) launch_span_copy(col.data, (const uint8_t*)blob.get(), (const long long*)src[k].get(), (const int32_t*)str_offs[k].get(), rows, (uint8_t*)bytes.get(), stream);
       set_varlen(c, {str_offs[k], bytes, total});
     } else if (t == DType::Bool) {
-      BufferPtr bits = device_alloc((size_t)(rows + 7) / 8 + 1);
-      if (rows) launch_pack_bits((const uint8_t*)values[k].get(), rows, (uint8_t*)bits.get(), nullptr, stream);
-      c.data = (const uint8_t*)bits.get(); c.data_bytes = (rows + 7) / 8; c.owners = {bits, values[k]};
+      set_bool_values(c, values[k], rows, stream);
     } else {
       c.data = (const uint8_t*)values[k].get(); c.data_bytes = rows * fixed_width(t); c.owners = {values[k]};
     }

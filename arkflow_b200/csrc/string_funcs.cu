@@ -6,6 +6,7 @@
 // empty strings and the result is never NULL.  Runs after the row kernels on the surviving rows:
 // lengths → exclusive scan → one thread per row writes its parts.
 #include "agg_acc.cuh"
+#include "bitmap.cuh"
 #include "engine.h"
 #include "stage_store.cuh"
 #include "varlen.h"
@@ -49,11 +50,10 @@ __device__ __forceinline__ int format_i64(long long v, uint8_t* out) {
 // bytes of part p for row r: *src points at them (literal / column bytes) or they are rendered into scratch
 __device__ __forceinline__ int part_len(const ConcatPartView& p, int64_t r, const uint8_t** src, uint8_t* scratch) {
   if (p.kind == PART_LITERAL) { *src = p.data; return p.lit_len; }
-  if (p.validity) { const int64_t b = r + p.validity_bit0; if (!((p.validity[b >> 3] >> (b & 7)) & 1)) return 0; }
+  if (p.validity && !bit_get(p.validity, r + p.validity_bit0)) return 0;
   if (p.kind == PART_INT64) { *src = scratch; return format_i64(reinterpret_cast<const long long*>(p.data)[r], scratch); }
   if (p.kind == PART_BOOL) {
-    const int64_t b = r + p.data_bit0;
-    const bool t = (p.data[b >> 3] >> (b & 7)) & 1;
+    const bool t = bit_get(p.data, r + p.data_bit0);
     const char* w = t ? "true" : "false";
     const int n = t ? 4 : 5;
     for (int i = 0; i < n; ++i) scratch[i] = (uint8_t)w[i];

@@ -1,5 +1,6 @@
 // vm.cuh — device-side interpreter for VmProgram (see vm.h for the semantics being restated).
 #pragma once
+#include "bitmap.cuh"
 #include "vm.h"
 
 namespace ark {
@@ -8,14 +9,6 @@ struct VmVal {
   uint64_t bits;
   bool valid;
 };
-
-__device__ __forceinline__ bool bit_get(const uint8_t* bm, int64_t i) {
-  return (bm[i >> 3] >> (i & 7)) & 1;
-}
-
-__device__ __forceinline__ bool col_valid(const ColView& c, int64_t row) {
-  return c.validity == nullptr || bit_get(c.validity, row + c.validity_bit0);
-}
 
 // IEEE-754 totalOrder key: monotone map from f64 bits to int64 (arrow-rs f64::total_cmp).
 __device__ __forceinline__ int64_t f64_total_key(uint64_t bits) {
