@@ -346,6 +346,9 @@ std::unique_ptr<Processor> make_arrow_to_json(const char* config_json) {
 }
 
 Batch arrow_to_json_device(const Processor& proc, Batch& in, cudaStream_t stream) {
+  std::vector<Column*> all;  // the byte extents of a device import's strings (a host import knows them: nothing to launch)
+  for (auto& c : in.cols) all.push_back(&c);
+  resolve_varlen_extents_many(all, stream);
   const auto& ap = static_cast<const ArrowToJsonProcessor&>(proc);
   const int64_t n = in.num_rows;
   AjParams P;

@@ -978,10 +978,7 @@ void export_host(const Batch& b, cudaStream_t stream, ArrowArray* out, ArrowSche
   export_schema(b, out_schema);
 }
 
-void export_device(const Batch& b, ArrowDeviceArray* out, ArrowSchema* out_schema, StreamLease* caller_lease) {
-  std::unique_ptr<StreamLease> own;
-  if (!caller_lease) own = std::make_unique<StreamLease>();
-  StreamLease& lease = caller_lease ? *caller_lease : *own;
+void export_device(const Batch& b, ArrowDeviceArray* out, ArrowSchema* out_schema, StreamLease& lease) {
   std::vector<ExportCol> cols;
   for (auto& c : b.cols) cols.push_back(normalise_for_export(c, false, lease.s));
   memset(out, 0, sizeof(*out));

@@ -169,9 +169,10 @@ void export_schema(const Batch& b, ArrowSchema* out);
 void export_empty_schema(ArrowSchema* out);  // RecordBatch::new_empty(Schema::empty()), sql.rs:137-139
 void export_host(const Batch& b, cudaStream_t stream, ArrowArray* out, ArrowSchema* out_schema,
                  int64_t* d2h_bytes = nullptr);
-// Device export queues its few normalising kernels on `lease`'s stream (a lease of its own when null) and ends with that
-// stream's last synchronize.
-void export_device(const Batch& b, ArrowDeviceArray* out, ArrowSchema* out_schema, StreamLease* lease = nullptr);
+// Device export queues its few normalising kernels (offset rebase, bitmap realignment) on the stream of the lease that
+// produced `b`, after the work that produced it, and ends with that stream's last synchronize: the caller queues nothing
+// more on it.
+void export_device(const Batch& b, ArrowDeviceArray* out, ArrowSchema* out_schema, StreamLease& lease);
 
 // Moves an ArrowArray into shared ownership: the returned pointer releases it when dropped.
 BufferPtr adopt_array(ArrowArray* arr);

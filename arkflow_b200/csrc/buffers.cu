@@ -22,7 +22,7 @@
 #include <deque>
 #include <thread>
 
-#include "engine.h"
+#include "abi.h"
 #include "json_mini.h"
 
 using namespace ark;
@@ -151,13 +151,6 @@ struct ark_buf {
 };
 
 namespace {
-
-template <typename F>
-int guarded(F&& f) {
-  try { f(); return ARK_OK; }
-  catch (const ArkError& e) { set_last_error(e.what()); return e.code; }
-  catch (const std::exception& e) { set_last_error(e.what()); return ARK_ERR_PROCESS; }
-}
 
 Batch concat_named(std::vector<Batch>& bs, cudaStream_t s) {
   Batch r = concat_device(bs, s);
@@ -293,8 +286,7 @@ int ark_buffer_write(ark_buf_t* b, ArrowArray* in, ArrowSchema* in_schema, const
   BufferPtr in_owner = adopt_array(in);
   return guarded([&] {
     if (!b) fail(ARK_ERR_PROCESS, "null buffer");
-    const ArrowArray* arr = (const ArrowArray*)in_owner.get();
-    if (!arr) fail(ARK_ERR_PROCESS, "input array already released");
+    const ArrowArray* arr = adopted(in_owner);
     StreamLease lease;
     Batch batch = import_host(arr, in_schema, nullptr, lease.s, nullptr, true);  // the window lives in HBM from here on
     ARK_CUDA(cudaStreamSynchronize(lease.s));
@@ -308,9 +300,7 @@ int ark_buffer_write_device(ark_buf_t* b, ArrowDeviceArray* in, ArrowSchema* in_
   BufferPtr in_owner = adopt_array(&in->array);
   return guarded([&] {
     if (!b) fail(ARK_ERR_PROCESS, "null buffer");
-    if (!in_owner) fail(ARK_ERR_PROCESS, "input array already released");
-    ArrowDeviceArray view = *in;
-    view.array = *(const ArrowArray*)in_owner.get();
+    ArrowDeviceArray view = device_view(*in, in_owner);
     Batch batch = import_device(&view, in_schema, nullptr, in_owner, true);
     buffer_enqueue(b, std::move(batch), input_name, ack_token);
   });
@@ -320,18 +310,15 @@ int ark_buffer_write_device(ark_buf_t* b, ArrowDeviceArray* in, ArrowSchema* in_
 static int buffer_read_impl(ark_buf_t* b, ArrowArray* out_host, ArrowDeviceArray* out_dev, ArrowSchema* out_schema, uint64_t* acks, int64_t acks_cap,
                             int64_t* n_acks) {
   return guarded([&] {
+    if (out_host) zero_out(out_host, out_schema); else zero_out(out_dev, out_schema);
     if (!b) fail(ARK_ERR_PROCESS, "null buffer");
-    ArrowArray* out = out_host ? out_host : &out_dev->array;
-    if (out_host) memset(out_host, 0, sizeof(*out_host)); else memset(out_dev, 0, sizeof(*out_dev));
-    if (out_schema) memset(out_schema, 0, sizeof(*out_schema));
     if (n_acks) *n_acks = 0;
     std::vector<uint64_t> got_acks;
     StreamLease lease;
-    auto export_host = [&](Batch& r, cudaStream_t s_, ArrowArray*, ArrowSchema* sch) {  // shadows ark::export_host below
-      if (out_host) ark::export_host(r, s_, out_host, sch);
-      else { ARK_CUDA(cudaStreamSynchronize(s_)); ark::export_device(r, out_dev, sch); }
+    auto export_window = [&](const Batch& r) {
+      if (out_host) export_host(r, lease.s, out_host, out_schema);
+      else export_device(r, out_dev, out_schema, lease);
     };
-    (void)out;
     if (b->kind == ark_buf::Memory) {
       std::vector<Batch> bs;
       {
@@ -347,8 +334,7 @@ static int buffer_read_impl(ark_buf_t* b, ArrowArray* out_host, ArrowDeviceArray
         }
         b->queued_rows = 0;
       }
-      Batch r = concat_device(bs, lease.s);
-      export_host(r, lease.s, out, out_schema);
+      export_window(concat_device(bs, lease.s));
     } else if (b->kind == ark_buf::Sliding) {
       std::vector<Batch> bs;
       {
@@ -364,8 +350,7 @@ static int buffer_read_impl(ark_buf_t* b, ArrowArray* out_host, ArrowDeviceArray
         }
         for (uint32_t i = 0; i < b->slide_size && !b->queue.empty(); ++i) b->queue.pop_front();  // :144-148
       }
-      Batch r = concat_device(bs, lease.s);
-      export_host(r, lease.s, out, out_schema);
+      export_window(concat_device(bs, lease.s));
     } else {
       std::vector<std::string> names;
       std::vector<std::deque<Queued>> queues;
@@ -384,10 +369,8 @@ static int buffer_read_impl(ark_buf_t* b, ArrowArray* out_host, ArrowDeviceArray
       }
       bool empty_schema = false;
       Batch r = process_window(b, names, queues, got_acks, &empty_schema, lease.s);
-      if (empty_schema) {  // RecordBatch::new_empty(Schema::empty()), join.rs:108
-        Batch e;
-        export_host(e, lease.s, out, out_schema);
-      } else export_host(r, lease.s, out, out_schema);
+      if (empty_schema) r = Batch();  // RecordBatch::new_empty(Schema::empty()), join.rs:108
+      export_window(r);
     }
     if ((int64_t)got_acks.size() > acks_cap) fail(ARK_ERR_PROCESS, "ack array too small: need " + std::to_string(got_acks.size()));
     for (size_t i = 0; i < got_acks.size(); ++i) acks[i] = got_acks[i];
@@ -462,11 +445,9 @@ static void batcher_flush_locked(ark_batcher* b, ArrowArray* out, ArrowSchema* o
 int ark_batch_process(ark_batcher_t* b, ArrowArray* in, ArrowSchema* in_schema, ArrowArray* out, ArrowSchema* out_schema) {
   BufferPtr in_owner = adopt_array(in);
   return guarded([&] {
+    zero_out(out, out_schema);
     if (!b) fail(ARK_ERR_PROCESS, "null batch processor");
-    memset(out, 0, sizeof(*out));
-    if (out_schema) memset(out_schema, 0, sizeof(*out_schema));
-    const ArrowArray* arr = (const ArrowArray*)in_owner.get();
-    if (!arr) fail(ARK_ERR_PROCESS, "input array already released");
+    const ArrowArray* arr = adopted(in_owner);
     Batch batch;
     {
       StreamLease lease;
@@ -483,9 +464,8 @@ int ark_batch_process(ark_batcher_t* b, ArrowArray* in, ArrowSchema* in_schema, 
 
 int ark_batch_flush(ark_batcher_t* b, ArrowArray* out, ArrowSchema* out_schema) {
   return guarded([&] {
+    zero_out(out, out_schema);
     if (!b) fail(ARK_ERR_PROCESS, "null batch processor");
-    memset(out, 0, sizeof(*out));
-    if (out_schema) memset(out_schema, 0, sizeof(*out_schema));
     std::lock_guard<std::mutex> l(b->mu);
     batcher_flush_locked(b, out, out_schema);
   });

@@ -1,45 +1,78 @@
 // capi.cu — extern "C" entry points declared in include/arkflow_b200.h.
-#include <cstring>
-
 #include <chrono>
 #include <map>
 #include <mutex>
 
-#include "engine.h"
+#include "abi.h"
 
 using namespace ark;
 
-struct ark_proc {
-  std::unique_ptr<Processor> impl;
-};
-
 namespace {
 
-template <typename F>
-int guarded(F&& f) {
-  try {
-    f();
-    return ARK_OK;
-  } catch (const ArkError& e) {
-    set_last_error(e.what());
-    return e.code;
-  } catch (const std::bad_alloc&) {
-    set_last_error("out of host memory");
-    return ARK_ERR_PROCESS;
-  } catch (const std::exception& e) {
-    set_last_error(e.what());
-    return ARK_ERR_PROCESS;
-  }
+template <typename Make>
+int create_proc(Make make, const char* config_json, ark_proc_t** out) {
+  return guarded([&] {
+    if (!out) fail(ARK_ERR_PROCESS, "null output handle");
+    *out = nullptr;
+    auto p = make(config_json);
+    auto* h = new ark_proc();
+    h->impl = std::move(p);
+    *out = h;
+  });
 }
 
-SqlProcessor* as_sql(ark_proc_t* p) {
-  if (!p || !p->impl || strcmp(p->impl->type(), "sql") != 0) fail(ARK_ERR_PROCESS, "handle is not a sql processor");
-  return static_cast<SqlProcessor*>(p->impl.get());
+// What the four codec processors' entry points differ in (processor/json.rs:42-113, processor/protobuf.rs:98-148).
+struct Codec {
+  const char* type;
+  const std::string& (*value_field)(const Processor&);  // the one column imported; nullptr: every column
+  bool none_on_empty;                                    // an empty input is ProcessResult::None (protobuf.rs:101-103)
+  bool codec_types;                                      // see import_host
+  Batch (*run)(const Processor&, Batch&, cudaStream_t);
+};
+
+const Codec kJsonToArrow{"json_to_arrow", json_to_arrow_value_field, false, false, json_to_arrow_device};
+const Codec kArrowToJson{"arrow_to_json", nullptr, false, false, arrow_to_json_device};
+const Codec kProtobufToArrow{"protobuf_to_arrow", protobuf_to_arrow_value_field, true, false, protobuf_to_arrow_device};
+const Codec kArrowToProtobuf{"arrow_to_protobuf", nullptr, true, true, arrow_to_protobuf_device};
+
+std::vector<bool> value_field_mask(const Codec& c, const Processor& p, const ArrowSchema* schema) {
+  std::vector<Field> fields = schema_fields(schema);
+  std::vector<bool> m(fields.size(), false);
+  for (size_t i = 0; i < fields.size(); ++i) if (fields[i].name == c.value_field(p)) m[i] = true;
+  return m;
 }
 
-void set_none(ArrowArray* out, ArrowSchema* out_schema) {
-  memset(out, 0, sizeof(*out));
-  if (out_schema) memset(out_schema, 0, sizeof(*out_schema));
+int codec_process(const Codec& c, ark_proc_t* p, ArrowArray* in, ArrowSchema* in_schema, ArrowArray* out, ArrowSchema* out_schema) {
+  BufferPtr in_owner = adopt_array(in);
+  return guarded([&] {
+    zero_out(out, out_schema);
+    Processor* proc = proc_of(p, c.type);
+    const ArrowArray* arr = adopted(in_owner);
+    if (c.none_on_empty && arr->length == 0) return;
+    std::vector<bool> mask;
+    if (c.value_field) mask = value_field_mask(c, *proc, in_schema);
+    StreamLease lease;
+    Batch b = import_host(arr, in_schema, c.value_field ? &mask : nullptr, lease.s, nullptr, c.codec_types);
+    Batch r = c.run(*proc, b, lease.s);
+    export_host(r, lease.s, out, out_schema);
+  });
+}
+
+int codec_process_device(const Codec& c, ark_proc_t* p, ArrowDeviceArray* in, ArrowSchema* in_schema, ArrowDeviceArray* out,
+                         ArrowSchema* out_schema) {
+  BufferPtr in_owner = adopt_array(&in->array);
+  return guarded([&] {
+    zero_out(out, out_schema);
+    Processor* proc = proc_of(p, c.type);
+    ArrowDeviceArray view = device_view(*in, in_owner);
+    if (c.none_on_empty && view.array.length == 0) return;
+    std::vector<bool> mask;
+    if (c.value_field) mask = value_field_mask(c, *proc, in_schema);
+    StreamLease lease;
+    Batch b = import_device(&view, in_schema, c.value_field ? &mask : nullptr, in_owner, c.codec_types);
+    Batch r = c.run(*proc, b, lease.s);
+    export_device(r, out, out_schema, lease);
+  });
 }
 
 }  // namespace
@@ -67,30 +100,19 @@ int ark_b200_device_count(int* out_count) {
 const char* ark_b200_version(void) { return "arkflow_b200 0.1.0 (sm_90a)"; }
 const char* ark_last_error(void) { return last_error_ref().c_str(); }
 
-int ark_sql_create(const char* config_json, ark_proc_t** out) {
-  return guarded([&] {
-    if (!out) fail(ARK_ERR_PROCESS, "null output handle");
-    *out = nullptr;
-    auto p = SqlProcessor::from_config(config_json);
-    auto* h = new ark_proc();
-    h->impl = std::move(p);
-    *out = h;
-  });
-}
+int ark_sql_create(const char* config_json, ark_proc_t** out) { return create_proc(SqlProcessor::from_config, config_json, out); }
 
 int ark_sql_process(ark_proc_t* p, ArrowArray* in, ArrowSchema* in_schema, ArrowArray* out, ArrowSchema* out_schema) {
-  BufferPtr in_owner = adopt_array(in);  // moved in: released on every path
+  BufferPtr in_owner = adopt_array(in);
   return guarded([&] {
+    zero_out(out, out_schema);
     SqlProcessor* sp = as_sql(p);
-    const ArrowArray* arr = (const ArrowArray*)in_owner.get();
-    if (!arr) fail(ARK_ERR_PROCESS, "input array already released");
-    if (arr->length == 0) { set_none(out, out_schema); return; }  // ProcessResult::None, sql.rs:211-213
-    std::vector<Field> fields = schema_fields(in_schema);
-    auto plan = sp->plan_for(fields);
-    std::vector<bool> mask = needed_mask(*plan, fields.size());
+    const ArrowArray* arr = adopted(in_owner);
+    if (arr->length == 0) return;  // ProcessResult::None, sql.rs:211-213
+    auto bound = sp->bind(in_schema);
     StreamLease lease;
-    Batch b = import_host(arr, in_schema, &mask, lease.s);
-    Batch r = sp->execute(*plan, b, lease.s);
+    Batch b = import_host(arr, in_schema, &bound->mask, lease.s);
+    Batch r = sp->execute(*bound->plan, b, lease.s);
     export_host(r, lease.s, out, out_schema);
   });
 }
@@ -99,11 +121,10 @@ int ark_sql_process_device(ark_proc_t* p, ArrowDeviceArray* in, ArrowSchema* in_
                            ArrowSchema* out_schema) {
   BufferPtr in_owner = adopt_array(&in->array);
   return guarded([&] {
+    zero_out(out, out_schema);
     SqlProcessor* sp = as_sql(p);
-    if (!in_owner) fail(ARK_ERR_PROCESS, "input array already released");
-    ArrowDeviceArray view = *in;
-    view.array = *(const ArrowArray*)in_owner.get();
-    if (view.array.length == 0) { memset(out, 0, sizeof(*out)); if (out_schema) memset(out_schema, 0, sizeof(*out_schema)); return; }
+    ArrowDeviceArray view = device_view(*in, in_owner);
+    if (view.array.length == 0) return;
     const bool trace = trace_enabled();  // per-phase host time of this entry point, to stderr
     auto now = [] { return std::chrono::steady_clock::now(); };
     auto us = [](std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b) {
@@ -118,7 +139,7 @@ int ark_sql_process_device(ark_proc_t* p, ArrowDeviceArray* in, ArrowSchema* in_
     const auto t2 = now();
     Batch r = sp->execute(*bound->plan, b, lease.s);
     const auto t3 = now();
-    export_device(r, out, out_schema, &lease);
+    export_device(r, out, out_schema, lease);
     const auto t4 = now();
     // the input's release (an outside callback) runs here, unless an exported column still aliases it
     r = Batch();
@@ -140,22 +161,19 @@ int ark_sql_partial_aggregate_device(ark_proc_t* p, ArrowDeviceArray* in, ArrowS
                                      ArrowDeviceArray* out, ArrowSchema* out_schema, int64_t* part_rows) {
   BufferPtr in_owner = adopt_array(&in->array);
   return guarded([&] {
+    zero_out(out, out_schema);
     SqlProcessor* sp = as_sql(p);
-    if (!in_owner) fail(ARK_ERR_PROCESS, "input array already released");
+    ArrowDeviceArray view = device_view(*in, in_owner);
     if (n_parts < 1) fail(ARK_ERR_PROCESS, "n_parts must be >= 1");
-    ArrowDeviceArray view = *in;
-    view.array = *(const ArrowArray*)in_owner.get();
-    std::vector<Field> fields = schema_fields(in_schema);
-    auto plan = sp->plan_for(fields);
-    if (plan->kind != Plan::Aggregate) fail(ARK_ERR_PROCESS, "partial aggregate requested for a query without aggregation");
-    std::vector<bool> mask = needed_mask(*plan, fields.size());
+    auto bound = sp->bind(in_schema);
+    if (bound->plan->kind != Plan::Aggregate) fail(ARK_ERR_PROCESS, "partial aggregate requested for a query without aggregation");
     StreamLease lease;
-    Batch b = import_device(&view, in_schema, &mask, in_owner);
+    Batch b = import_device(&view, in_schema, &bound->mask, in_owner, false, &bound->fields);
     std::vector<int64_t> rows;
     ExportAllocScope exported;  // the partial states are published to the other ranks over CUDA IPC
-    Batch r = run_partial_aggregate(*plan, b, n_parts, rows, lease.s);
+    Batch r = run_partial_aggregate(*bound->plan, b, n_parts, rows, lease.s);
     for (int i = 0; i < n_parts; ++i) part_rows[i] = rows[i];
-    export_device(r, out, out_schema);
+    export_device(r, out, out_schema, lease);
   });
 }
 
@@ -163,16 +181,15 @@ int ark_sql_final_aggregate_device(ark_proc_t* p, ArrowDeviceArray* in, ArrowSch
                                    ArrowSchema* out_schema) {
   BufferPtr in_owner = adopt_array(&in->array);
   return guarded([&] {
+    zero_out(out, out_schema);
     SqlProcessor* sp = as_sql(p);
-    if (!in_owner) fail(ARK_ERR_PROCESS, "input array already released");
-    ArrowDeviceArray view = *in;
-    view.array = *(const ArrowArray*)in_owner.get();
+    ArrowDeviceArray view = device_view(*in, in_owner);
     auto plan = sp->last_aggregate_plan();
     if (!plan) fail(ARK_ERR_PROCESS, "final aggregate called before any partial aggregate bound the query");
     StreamLease lease;
     Batch b = import_device(&view, in_schema, nullptr, in_owner);
     Batch r = run_final_aggregate(*plan, b, lease.s);
-    export_device(r, out, out_schema);
+    export_device(r, out, out_schema, lease);
   });
 }
 
@@ -197,6 +214,7 @@ int ark_sql_process_tables(ark_proc_t* p, int n_tables, const char* const* names
   std::vector<BufferPtr> owners;
   for (int i = 0; i < n_tables; ++i) owners.push_back(adopt_array(&ins[i]));
   return guarded([&] {
+    zero_out(out, out_schema);
     SqlProcessor* sp = as_sql(p);
     StreamLease lease;
     std::vector<std::string> nm;
@@ -205,7 +223,7 @@ int ark_sql_process_tables(ark_proc_t* p, int n_tables, const char* const* names
     for (int i = 0; i < n_tables; ++i) {
       nm.push_back(names[i]);
       schemas.push_back(schema_fields(&in_schemas[i]));
-      tables.push_back(import_host((const ArrowArray*)owners[i].get(), &in_schemas[i], nullptr, lease.s));
+      tables.push_back(import_host(adopted(owners[i]), &in_schemas[i], nullptr, lease.s));
     }
     Batch r = run_tables(sp, nm, schemas, tables, lease.s);
     export_host(r, lease.s, out, out_schema);
@@ -217,6 +235,7 @@ int ark_sql_process_tables_device(ark_proc_t* p, int n_tables, const char* const
   std::vector<BufferPtr> owners;
   for (int i = 0; i < n_tables; ++i) owners.push_back(adopt_array(&ins[i].array));
   return guarded([&] {
+    zero_out(out, out_schema);
     SqlProcessor* sp = as_sql(p);
     StreamLease lease;
     std::vector<std::string> nm;
@@ -225,12 +244,11 @@ int ark_sql_process_tables_device(ark_proc_t* p, int n_tables, const char* const
     for (int i = 0; i < n_tables; ++i) {
       nm.push_back(names[i]);
       schemas.push_back(schema_fields(&in_schemas[i]));
-      ArrowDeviceArray view = ins[i];
-      view.array = *(const ArrowArray*)owners[i].get();
+      ArrowDeviceArray view = device_view(ins[i], owners[i]);
       tables.push_back(import_device(&view, &in_schemas[i], nullptr, owners[i]));
     }
     Batch r = run_tables(sp, nm, schemas, tables, lease.s);
-    export_device(r, out, out_schema);
+    export_device(r, out, out_schema, lease);
   });
 }
 
@@ -238,206 +256,51 @@ int ark_hash_partition_device(ArrowDeviceArray* in, ArrowSchema* in_schema, cons
                               ArrowDeviceArray* out, ArrowSchema* out_schema, int64_t* part_rows) {
   BufferPtr in_owner = adopt_array(&in->array);
   return guarded([&] {
-    if (!in_owner) fail(ARK_ERR_PROCESS, "input array already released");
-    ArrowDeviceArray view = *in;
-    view.array = *(const ArrowArray*)in_owner.get();
+    zero_out(out, out_schema);
+    ArrowDeviceArray view = device_view(*in, in_owner);
     StreamLease lease;
     Batch b = import_device(&view, in_schema, nullptr, in_owner);
     std::vector<int64_t> rows;
     Batch r = hash_partition(b, key_column ? key_column : "", n_parts, rows, lease.s);
     for (int i = 0; i < n_parts; ++i) part_rows[i] = rows[i];
-    export_device(r, out, out_schema);
+    export_device(r, out, out_schema, lease);
   });
 }
 
-int ark_json_to_arrow_create(const char* config_json, ark_proc_t** out) {
-  return guarded([&] {
-    if (!out) fail(ARK_ERR_PROCESS, "null output handle");
-    *out = nullptr;
-    auto p = make_json_to_arrow(config_json);
-    auto* h = new ark_proc();
-    h->impl = std::move(p);
-    *out = h;
-  });
-}
-
-static Processor* as_json(ark_proc_t* p) {
-  if (!p || !p->impl || strcmp(p->impl->type(), "json_to_arrow") != 0) fail(ARK_ERR_PROCESS, "handle is not a json_to_arrow processor");
-  return p->impl.get();
-}
-
-static std::vector<bool> json_mask(const Processor& jp, const std::vector<Field>& fields) {
-  std::vector<bool> m(fields.size(), false);
-  for (size_t i = 0; i < fields.size(); ++i) if (fields[i].name == json_to_arrow_value_field(jp)) m[i] = true;
-  return m;
-}
-
+int ark_json_to_arrow_create(const char* config_json, ark_proc_t** out) { return create_proc(make_json_to_arrow, config_json, out); }
 int ark_json_to_arrow_process(ark_proc_t* p, ArrowArray* in, ArrowSchema* in_schema, ArrowArray* out, ArrowSchema* out_schema) {
-  BufferPtr in_owner = adopt_array(in);
-  return guarded([&] {
-    Processor* jp = as_json(p);
-    const ArrowArray* arr = (const ArrowArray*)in_owner.get();
-    if (!arr) fail(ARK_ERR_PROCESS, "input array already released");
-    std::vector<Field> fields = schema_fields(in_schema);
-    std::vector<bool> mask = json_mask(*jp, fields);
-    StreamLease lease;
-    Batch b = import_host(arr, in_schema, &mask, lease.s);
-    Batch r = json_to_arrow_device(*jp, b, lease.s);
-    export_host(r, lease.s, out, out_schema);
-  });
+  return codec_process(kJsonToArrow, p, in, in_schema, out, out_schema);
 }
-
 int ark_json_to_arrow_process_device(ark_proc_t* p, ArrowDeviceArray* in, ArrowSchema* in_schema, ArrowDeviceArray* out,
                                      ArrowSchema* out_schema) {
-  BufferPtr in_owner = adopt_array(&in->array);
-  return guarded([&] {
-    Processor* jp = as_json(p);
-    if (!in_owner) fail(ARK_ERR_PROCESS, "input array already released");
-    ArrowDeviceArray view = *in;
-    view.array = *(const ArrowArray*)in_owner.get();
-    std::vector<Field> fields = schema_fields(in_schema);
-    std::vector<bool> mask = json_mask(*jp, fields);
-    StreamLease lease;
-    Batch b = import_device(&view, in_schema, &mask, in_owner);
-    Batch r = json_to_arrow_device(*jp, b, lease.s);
-    export_device(r, out, out_schema);
-  });
+  return codec_process_device(kJsonToArrow, p, in, in_schema, out, out_schema);
 }
 
-int ark_arrow_to_json_create(const char* config_json, ark_proc_t** out) {
-  return guarded([&] {
-    if (!out) fail(ARK_ERR_PROCESS, "null output handle");
-    *out = nullptr;
-    auto p = make_arrow_to_json(config_json);
-    auto* h = new ark_proc();
-    h->impl = std::move(p);
-    *out = h;
-  });
-}
-
+int ark_arrow_to_json_create(const char* config_json, ark_proc_t** out) { return create_proc(make_arrow_to_json, config_json, out); }
 int ark_arrow_to_json_process(ark_proc_t* p, ArrowArray* in, ArrowSchema* in_schema, ArrowArray* out, ArrowSchema* out_schema) {
-  BufferPtr in_owner = adopt_array(in);
-  return guarded([&] {
-    if (!p || !p->impl || strcmp(p->impl->type(), "arrow_to_json") != 0) fail(ARK_ERR_PROCESS, "handle is not an arrow_to_json processor");
-    const ArrowArray* arr = (const ArrowArray*)in_owner.get();
-    if (!arr) fail(ARK_ERR_PROCESS, "input array already released");
-    StreamLease lease;
-    Batch b = import_host(arr, in_schema, nullptr, lease.s);
-    Batch r = arrow_to_json_device(*p->impl, b, lease.s);
-    export_host(r, lease.s, out, out_schema);
-  });
+  return codec_process(kArrowToJson, p, in, in_schema, out, out_schema);
 }
-
 int ark_arrow_to_json_process_device(ark_proc_t* p, ArrowDeviceArray* in, ArrowSchema* in_schema, ArrowDeviceArray* out,
                                      ArrowSchema* out_schema) {
-  BufferPtr in_owner = adopt_array(&in->array);
-  return guarded([&] {
-    if (!p || !p->impl || strcmp(p->impl->type(), "arrow_to_json") != 0) fail(ARK_ERR_PROCESS, "handle is not an arrow_to_json processor");
-    if (!in_owner) fail(ARK_ERR_PROCESS, "input array already released");
-    ArrowDeviceArray view = *in;
-    view.array = *(const ArrowArray*)in_owner.get();
-    StreamLease lease;
-    Batch b = import_device(&view, in_schema, nullptr, in_owner);
-    std::vector<Column*> all;
-    for (auto& c : b.cols) all.push_back(&c);
-    resolve_varlen_extents_many(all, lease.s);
-    Batch r = arrow_to_json_device(*p->impl, b, lease.s);
-    export_device(r, out, out_schema);
-  });
-}
-
-// ---- protobuf_to_arrow / arrow_to_protobuf (processor/protobuf.rs:98-148) --------------------------------------
-static int create_proc(std::unique_ptr<Processor> (*make)(const char*), const char* config_json, ark_proc_t** out) {
-  return guarded([&] {
-    if (!out) fail(ARK_ERR_PROCESS, "null output handle");
-    *out = nullptr;
-    auto p = make(config_json);
-    auto* h = new ark_proc();
-    h->impl = std::move(p);
-    *out = h;
-  });
-}
-
-static Processor* as_type(ark_proc_t* p, const char* type) {
-  if (!p || !p->impl || strcmp(p->impl->type(), type) != 0) fail(ARK_ERR_PROCESS, std::string("handle is not a ") + type + " processor");
-  return p->impl.get();
+  return codec_process_device(kArrowToJson, p, in, in_schema, out, out_schema);
 }
 
 int ark_protobuf_to_arrow_create(const char* config_json, ark_proc_t** out) { return create_proc(make_protobuf_to_arrow, config_json, out); }
-
-static std::vector<bool> protobuf_mask(const Processor& pp, const std::vector<Field>& fields) {
-  std::vector<bool> m(fields.size(), false);
-  for (size_t i = 0; i < fields.size(); ++i) if (fields[i].name == protobuf_to_arrow_value_field(pp)) m[i] = true;
-  return m;
-}
-
 int ark_protobuf_to_arrow_process(ark_proc_t* p, ArrowArray* in, ArrowSchema* in_schema, ArrowArray* out, ArrowSchema* out_schema) {
-  BufferPtr in_owner = adopt_array(in);
-  return guarded([&] {
-    Processor* pp = as_type(p, "protobuf_to_arrow");
-    const ArrowArray* arr = (const ArrowArray*)in_owner.get();
-    if (!arr) fail(ARK_ERR_PROCESS, "input array already released");
-    if (arr->length == 0) { set_none(out, out_schema); return; }  // ProcessResult::None, protobuf.rs:101-103
-    std::vector<Field> fields = schema_fields(in_schema);
-    std::vector<bool> mask = protobuf_mask(*pp, fields);
-    StreamLease lease;
-    Batch b = import_host(arr, in_schema, &mask, lease.s);
-    Batch r = protobuf_to_arrow_device(*pp, b, lease.s);
-    export_host(r, lease.s, out, out_schema);
-  });
+  return codec_process(kProtobufToArrow, p, in, in_schema, out, out_schema);
 }
-
 int ark_protobuf_to_arrow_process_device(ark_proc_t* p, ArrowDeviceArray* in, ArrowSchema* in_schema, ArrowDeviceArray* out,
                                          ArrowSchema* out_schema) {
-  BufferPtr in_owner = adopt_array(&in->array);
-  return guarded([&] {
-    Processor* pp = as_type(p, "protobuf_to_arrow");
-    if (!in_owner) fail(ARK_ERR_PROCESS, "input array already released");
-    ArrowDeviceArray view = *in;
-    view.array = *(const ArrowArray*)in_owner.get();
-    if (view.array.length == 0) { memset(out, 0, sizeof(*out)); if (out_schema) memset(out_schema, 0, sizeof(*out_schema)); return; }
-    std::vector<Field> fields = schema_fields(in_schema);
-    std::vector<bool> mask = protobuf_mask(*pp, fields);
-    StreamLease lease;
-    Batch b = import_device(&view, in_schema, &mask, in_owner);
-    Batch r = protobuf_to_arrow_device(*pp, b, lease.s);
-    export_device(r, out, out_schema);
-  });
+  return codec_process_device(kProtobufToArrow, p, in, in_schema, out, out_schema);
 }
 
 int ark_arrow_to_protobuf_create(const char* config_json, ark_proc_t** out) { return create_proc(make_arrow_to_protobuf, config_json, out); }
-
 int ark_arrow_to_protobuf_process(ark_proc_t* p, ArrowArray* in, ArrowSchema* in_schema, ArrowArray* out, ArrowSchema* out_schema) {
-  BufferPtr in_owner = adopt_array(in);
-  return guarded([&] {
-    Processor* pp = as_type(p, "arrow_to_protobuf");
-    const ArrowArray* arr = (const ArrowArray*)in_owner.get();
-    if (!arr) fail(ARK_ERR_PROCESS, "input array already released");
-    if (arr->length == 0) { set_none(out, out_schema); return; }  // ProcessResult::None, protobuf.rs:101-103
-    StreamLease lease;
-    Batch b = import_host(arr, in_schema, nullptr, lease.s, nullptr, true);
-    Batch r = arrow_to_protobuf_device(*pp, b, lease.s);
-    export_host(r, lease.s, out, out_schema);
-  });
+  return codec_process(kArrowToProtobuf, p, in, in_schema, out, out_schema);
 }
-
 int ark_arrow_to_protobuf_process_device(ark_proc_t* p, ArrowDeviceArray* in, ArrowSchema* in_schema, ArrowDeviceArray* out,
                                          ArrowSchema* out_schema) {
-  BufferPtr in_owner = adopt_array(&in->array);
-  return guarded([&] {
-    Processor* pp = as_type(p, "arrow_to_protobuf");
-    if (!in_owner) fail(ARK_ERR_PROCESS, "input array already released");
-    ArrowDeviceArray view = *in;
-    view.array = *(const ArrowArray*)in_owner.get();
-    if (view.array.length == 0) { memset(out, 0, sizeof(*out)); if (out_schema) memset(out_schema, 0, sizeof(*out_schema)); return; }
-    StreamLease lease;
-    Batch b = import_device(&view, in_schema, nullptr, in_owner, true);
-    std::vector<Column*> all;
-    for (auto& c : b.cols) all.push_back(&c);
-    resolve_varlen_extents_many(all, lease.s);
-    Batch r = arrow_to_protobuf_device(*pp, b, lease.s);
-    export_device(r, out, out_schema);
-  });
+  return codec_process_device(kArrowToProtobuf, p, in, in_schema, out, out_schema);
 }
 
 // ---- expr::evaluate_expr (plugin/expr/mod.rs:92-122) ---------------------------------------------------
@@ -512,9 +375,9 @@ Batch evaluate_expr_on(const CachedExpr& ce, Batch& in, const std::vector<Field>
 int ark_expr_evaluate(const char* expr, ArrowArray* in, ArrowSchema* in_schema, ArrowArray* out, ArrowSchema* out_schema, int* is_scalar) {
   BufferPtr in_owner = adopt_array(in);
   return guarded([&] {
+    zero_out(out, out_schema);
     if (!expr || !out) fail(ARK_ERR_PROCESS, "null argument");
-    const ArrowArray* arr = (const ArrowArray*)in_owner.get();
-    if (!arr) fail(ARK_ERR_PROCESS, "input array already released");
+    const ArrowArray* arr = adopted(in_owner);
     CachedExpr ce = expr_processor(expr);
     if (is_scalar) *is_scalar = ce.scalar ? 1 : 0;
     std::vector<Field> fields = schema_fields(in_schema);
@@ -534,10 +397,9 @@ int ark_expr_evaluate_device(const char* expr, ArrowDeviceArray* in, ArrowSchema
                              int* is_scalar) {
   BufferPtr in_owner = adopt_array(&in->array);
   return guarded([&] {
+    zero_out(out, out_schema);
     if (!expr || !out) fail(ARK_ERR_PROCESS, "null argument");
-    if (!in_owner) fail(ARK_ERR_PROCESS, "input array already released");
-    ArrowDeviceArray view = *in;
-    view.array = *(const ArrowArray*)in_owner.get();
+    ArrowDeviceArray view = device_view(*in, in_owner);
     CachedExpr ce = expr_processor(expr);
     if (is_scalar) *is_scalar = ce.scalar ? 1 : 0;
     std::vector<Field> fields = schema_fields(in_schema);
@@ -549,8 +411,7 @@ int ark_expr_evaluate_device(const char* expr, ArrowDeviceArray* in, ArrowSchema
       b = import_device(&view, in_schema, &mask, in_owner);
     }
     Batch r = evaluate_expr_on(ce, b, fields, lease.s);
-    ARK_CUDA(cudaStreamSynchronize(lease.s));
-    export_device(r, out, out_schema);
+    export_device(r, out, out_schema, lease);
   });
 }
 

@@ -7,8 +7,8 @@
 // (SURVEY.md §8(d) config 5: 2 × 32 B/row for decoded S, 134 B/msg for raw Binary payloads).
 #include <algorithm>
 
+#include "abi.h"
 #include "bitmap.cuh"
-#include "engine.h"
 
 namespace ark {
 
@@ -304,37 +304,30 @@ using namespace ark;
 extern "C" int ark_concat_batches(int n, ArrowArray* ins, ArrowSchema* in_schemas, ArrowArray* out, ArrowSchema* out_schema) {
   std::vector<BufferPtr> owners;
   for (int i = 0; i < n; ++i) owners.push_back(adopt_array(&ins[i]));
-  try {
+  return guarded([&] {
+    zero_out(out, out_schema);
     if (n <= 0) fail(ARK_ERR_PROCESS, "Merge batches failed: no batches");
     StreamLease lease;
     std::vector<Batch> bs;
-    for (int i = 0; i < n; ++i) bs.push_back(import_host((const ArrowArray*)owners[i].get(), &in_schemas[i], nullptr, lease.s, nullptr, true));
+    for (int i = 0; i < n; ++i) bs.push_back(import_host(adopted(owners[i]), &in_schemas[i], nullptr, lease.s, nullptr, true));
     Batch r = concat_device(bs, lease.s);
     export_host(r, lease.s, out, out_schema);
-    return ARK_OK;
-  } catch (const ArkError& e) {
-    set_last_error(e.what());
-    return e.code;
-  }
+  });
 }
 
 extern "C" int ark_concat_batches_device(int n, ArrowDeviceArray* ins, ArrowSchema* in_schemas, ArrowDeviceArray* out, ArrowSchema* out_schema) {
   std::vector<BufferPtr> owners;
   for (int i = 0; i < n; ++i) owners.push_back(adopt_array(&ins[i].array));
-  try {
+  return guarded([&] {
+    zero_out(out, out_schema);
     if (n <= 0) fail(ARK_ERR_PROCESS, "Merge batches failed: no batches");
     StreamLease lease;
     std::vector<Batch> bs;
     for (int i = 0; i < n; ++i) {
-      ArrowDeviceArray view = ins[i];
-      view.array = *(const ArrowArray*)owners[i].get();
+      ArrowDeviceArray view = device_view(ins[i], owners[i]);
       bs.push_back(import_device(&view, &in_schemas[i], nullptr, owners[i], true));
     }
     Batch r = concat_device(bs, lease.s);
-    export_device(r, out, out_schema);
-    return ARK_OK;
-  } catch (const ArkError& e) {
-    set_last_error(e.what());
-    return e.code;
-  }
+    export_device(r, out, out_schema, lease);
+  });
 }

@@ -22,8 +22,8 @@
 // Ordering: record stores → __threadfence_system() → grid-wide "last CTA" count → count → st.release.sys ready.  The
 // receiver polls ready with ld.acquire.sys.  Regions are double-buffered by step parity; before writing parity p of
 // step s a sender waits for ack ≥ s − 2 from every destination (always already true in lockstep operation).
+#include "abi.h"
 #include "agg_acc.cuh"
-#include "engine.h"
 #include "group_exchange.h"
 #include "hash_agg.cuh"
 #include "hashkey.cuh"
@@ -240,9 +240,6 @@ using namespace ark;
 struct ark_dist {
   DistCtx ctx;
 };
-struct ark_proc {
-  std::unique_ptr<Processor> impl;
-};
 
 namespace {
 
@@ -255,24 +252,12 @@ struct GxHandle {  // what ark_dist_export hands to the peers
   uint8_t ipc[64];
 };
 
-template <typename F>
-int gx_guarded(F&& f) {
-  try { f(); return ARK_OK; }
-  catch (const ArkError& e) { set_last_error(e.what()); return e.code; }
-  catch (const std::exception& e) { set_last_error(e.what()); return ARK_ERR_PROCESS; }
-}
-
-SqlProcessor* gx_sql(ark_proc_t* p) {
-  if (!p || !p->impl || strcmp(p->impl->type(), "sql") != 0) fail(ARK_ERR_PROCESS, "handle is not a sql processor");
-  return static_cast<SqlProcessor*>(p->impl.get());
-}
-
 }  // namespace
 
 extern "C" {
 
 int ark_dist_create(int rank, int world, int64_t region_bytes, ark_dist_t** out) {
-  return gx_guarded([&] {
+  return guarded([&] {
     if (!out) fail(ARK_ERR_PROCESS, "null output handle");
     *out = nullptr;
     if (world < 1 || world > GX_MAX_WORLD || rank < 0 || rank >= world) fail(ARK_ERR_CONFIG, "ark_dist_create: rank/world out of range (world <= 16)");
@@ -295,7 +280,7 @@ int ark_dist_create(int rank, int world, int64_t region_bytes, ark_dist_t** out)
 int64_t ark_dist_handle_bytes(void) { return (int64_t)sizeof(GxHandle); }
 
 int ark_dist_export(ark_dist_t* d, uint8_t* blob, int64_t blob_cap, int64_t* blob_size) {
-  return gx_guarded([&] {
+  return guarded([&] {
     if (!d || !blob) fail(ARK_ERR_PROCESS, "null argument");
     if (blob_size) *blob_size = (int64_t)sizeof(GxHandle);
     if (blob_cap < (int64_t)sizeof(GxHandle)) fail(ARK_ERR_PROCESS, "ark_dist_export: handle buffer too small");
@@ -312,7 +297,7 @@ int ark_dist_export(ark_dist_t* d, uint8_t* blob, int64_t blob_cap, int64_t* blo
 }
 
 int ark_dist_connect(ark_dist_t* d, const uint8_t* blobs, int64_t blob_stride) {
-  return gx_guarded([&] {
+  return guarded([&] {
     if (!d || !blobs) fail(ARK_ERR_PROCESS, "null argument");
     DistCtx& c = d->ctx;
     if (c.connected) fail(ARK_ERR_PROCESS, "ark_dist_connect: already connected");
@@ -348,7 +333,7 @@ int ark_dist_connect(ark_dist_t* d, const uint8_t* blobs, int64_t blob_stride) {
 }
 
 int ark_dist_stats(ark_dist_t* d, int64_t* out4) {
-  return gx_guarded([&] {
+  return guarded([&] {
     if (!d || !out4) fail(ARK_ERR_PROCESS, "null argument");
     std::lock_guard<std::mutex> l(d->ctx.mu);
     out4[0] = (int64_t)d->ctx.step; out4[1] = (int64_t)d->ctx.last_recv_records; out4[2] = (int64_t)d->ctx.last_groups;
@@ -367,31 +352,27 @@ void ark_dist_destroy(ark_dist_t* d) {
 
 int ark_sql_group_by_push_device(ark_proc_t* p, ark_dist_t* d, ArrowDeviceArray* in, ArrowSchema* in_schema) {
   BufferPtr in_owner = adopt_array(&in->array);
-  return gx_guarded([&] {
-    SqlProcessor* sp = gx_sql(p);
+  return guarded([&] {
+    SqlProcessor* sp = as_sql(p);
     if (!d || !d->ctx.connected) fail(ARK_ERR_PROCESS, "exchange context is not connected");
-    if (!in_owner) fail(ARK_ERR_PROCESS, "input array already released");
+    ArrowDeviceArray view = device_view(*in, in_owner);
     DistCtx& c = d->ctx;
     std::lock_guard<std::mutex> l(c.mu);
     if (c.pushed) fail(ARK_ERR_PROCESS, "ark_sql_group_by_push_device: the previous step has not been merged");
-    ArrowDeviceArray view = *in;
-    view.array = *(const ArrowArray*)in_owner.get();
-    std::vector<Field> fields = schema_fields(in_schema);
-    auto plan = sp->plan_for(fields);
-    if (plan->kind != Plan::Aggregate) fail(ARK_ERR_PROCESS, "not an aggregate query");
-    std::vector<bool> mask(fields.size(), false);
-    for (int col : plan->used_cols) mask[col] = true;
+    auto bound = sp->bind(in_schema);
+    if (bound->plan->kind != Plan::Aggregate) fail(ARK_ERR_PROCESS, "not an aggregate query");
     StreamLease lease;
-    Batch b = import_device(&view, in_schema, &mask, in_owner);
+    Batch b = import_device(&view, in_schema, &bound->mask, in_owner, false, &bound->fields);
     ++c.step;
     c.pushed = true;
-    run_group_by_push(*plan, b, c, lease.s);
+    run_group_by_push(*bound->plan, b, c, lease.s);
   });
 }
 
 int ark_sql_group_by_merge_device(ark_proc_t* p, ark_dist_t* d, ArrowDeviceArray* out, ArrowSchema* out_schema) {
-  return gx_guarded([&] {
-    SqlProcessor* sp = gx_sql(p);
+  return guarded([&] {
+    zero_out(out, out_schema);
+    SqlProcessor* sp = as_sql(p);
     if (!d || !d->ctx.connected) fail(ARK_ERR_PROCESS, "exchange context is not connected");
     DistCtx& c = d->ctx;
     std::lock_guard<std::mutex> l(c.mu);
@@ -403,7 +384,7 @@ int ark_sql_group_by_merge_device(ark_proc_t* p, ark_dist_t* d, ArrowDeviceArray
     Batch r;
     if (!run_group_by_merge(*plan, c, r, lease.s))
       fail(ARK_ERR_UNSUPPORTED, "device-side exchange: a GROUP BY key longer than 12 bytes cannot travel inline (use the descriptor exchange)");
-    export_device(r, out, out_schema);
+    export_device(r, out, out_schema, lease);
   });
 }
 

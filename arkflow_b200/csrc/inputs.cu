@@ -47,7 +47,7 @@
 
 #include "bitmap.h"
 #include "decimal.cuh"
-#include "engine.h"
+#include "abi.h"
 #include "json_mini.h"
 #include "utf8.cuh"
 #include "varlen.h"
@@ -57,13 +57,6 @@ using namespace ark;
 namespace {
 
 using Clock = std::chrono::steady_clock;
-
-template <typename F>
-int in_guarded(F&& f) {
-  try { f(); return ARK_OK; }
-  catch (const ArkError& e) { set_last_error(e.what()); return e.code; }
-  catch (const std::exception& e) { set_last_error(e.what()); return ARK_ERR_PROCESS; }
-}
 
 // humantime subset shared with buffers.cu's configs ("1ns", "10ms", "1s", "2m" …)
 std::chrono::nanoseconds parse_duration_in(const std::string& s) {
@@ -632,7 +625,7 @@ bool input_next(ark_input* in, Batch& out, cudaStream_t stream) {
 extern "C" {
 
 int ark_input_create(const char* type, const char* config_json, ark_input_t** out) {
-  return in_guarded([&] {
+  return guarded([&] {
     if (!out || !type) fail(ARK_ERR_PROCESS, "null argument");
     *out = nullptr;
     const std::string k = type;
@@ -701,7 +694,7 @@ int ark_input_create(const char* type, const char* config_json, ark_input_t** ou
 }
 
 int ark_input_connect(ark_input_t* in) {
-  return in_guarded([&] {
+  return guarded([&] {
     if (!in) fail(ARK_ERR_PROCESS, "null input");
     if (in->kind == ark_input::Generate) return;  // generate.rs:62-64
     std::lock_guard<std::mutex> l(in->mu);
@@ -742,23 +735,20 @@ int ark_input_connect(ark_input_t* in) {
 }
 
 int ark_input_read_device(ark_input_t* in, ArrowDeviceArray* out, ArrowSchema* out_schema) {
-  return in_guarded([&] {
+  return guarded([&] {
+    zero_out(out, out_schema);
     if (!in || !out) fail(ARK_ERR_PROCESS, "null argument");
-    memset(out, 0, sizeof(*out));
-    if (out_schema) memset(out_schema, 0, sizeof(*out_schema));
     StreamLease lease;
     Batch b;
     if (!input_next(in, b, lease.s)) fail(ARK_ERR_EOF, "EOF");
-    ARK_CUDA(cudaStreamSynchronize(lease.s));
-    export_device(b, out, out_schema);
+    export_device(b, out, out_schema, lease);
   });
 }
 
 int ark_input_read(ark_input_t* in, ArrowArray* out, ArrowSchema* out_schema) {
-  return in_guarded([&] {
+  return guarded([&] {
+    zero_out(out, out_schema);
     if (!in || !out) fail(ARK_ERR_PROCESS, "null argument");
-    memset(out, 0, sizeof(*out));
-    if (out_schema) memset(out_schema, 0, sizeof(*out_schema));
     StreamLease lease;
     Batch b;
     if (!input_next(in, b, lease.s)) fail(ARK_ERR_EOF, "EOF");
@@ -767,7 +757,7 @@ int ark_input_read(ark_input_t* in, ArrowArray* out, ArrowSchema* out_schema) {
 }
 
 int ark_input_close(ark_input_t* in) {
-  return in_guarded([&] {
+  return guarded([&] {
     if (!in) fail(ARK_ERR_PROCESS, "null input");
     std::lock_guard<std::mutex> l(in->mu);
     if (in->kind != ark_input::Generate) in->closed = true;  // file.rs:458-461 cancels the stream; generate.rs:93-95 is a no-op

@@ -11,7 +11,7 @@
 #include <map>
 #include <mutex>
 
-#include "engine.h"
+#include "abi.h"
 
 namespace ark {
 
@@ -170,31 +170,25 @@ extern "C" {
 
 int ark_ipc_export_device(ArrowDeviceArray* in, ArrowSchema* in_schema, uint8_t* blob, int64_t blob_cap, int64_t* blob_size) {
   BufferPtr in_owner = adopt_array(&in->array);
-  try {
-    if (!in_owner) fail(ARK_ERR_PROCESS, "input array already released");
-    ArrowDeviceArray view = *in;
-    view.array = *(const ArrowArray*)in_owner.get();
+  return guarded([&] {
+    ArrowDeviceArray view = device_view(*in, in_owner);
     Batch b = import_device(&view, in_schema, nullptr, in_owner);
     std::vector<uint8_t> out = ipc_export(b);
     if (blob_size) *blob_size = (int64_t)out.size();
     if ((int64_t)out.size() > blob_cap) fail(ARK_ERR_PROCESS, "ipc export: descriptor buffer too small");
     memcpy(blob, out.data(), out.size());
-    return ARK_OK;
-  } catch (const ArkError& e) { set_last_error(e.what()); return e.code; }
-  catch (const std::exception& e) { set_last_error(e.what()); return ARK_ERR_PROCESS; }
+  });
 }
 
 int ark_ipc_concat_slices_device(int n_src, const uint8_t* const* blobs, const int64_t* blob_sizes, const int64_t* row0, const int64_t* n_rows,
                                  ArrowDeviceArray* out, ArrowSchema* out_schema) {
-  try {
+  return guarded([&] {
+    zero_out(out, out_schema);
     if (n_src <= 0 || !blobs || !blob_sizes || !row0 || !n_rows || !out) fail(ARK_ERR_PROCESS, "null argument");
     StreamLease lease;
     Batch r = ipc_concat_slices(n_src, blobs, blob_sizes, row0, n_rows, lease.s);
-    ARK_CUDA(cudaStreamSynchronize(lease.s));
-    export_device(r, out, out_schema);
-    return ARK_OK;
-  } catch (const ArkError& e) { set_last_error(e.what()); return e.code; }
-  catch (const std::exception& e) { set_last_error(e.what()); return ARK_ERR_PROCESS; }
+    export_device(r, out, out_schema, lease);
+  });
 }
 
 }  // extern "C"

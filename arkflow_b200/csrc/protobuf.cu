@@ -569,6 +569,9 @@ Batch protobuf_to_arrow_device(const Processor& proc, Batch& in, cudaStream_t st
 
 // `in` was imported with codec_types (Int32 / UInt32 / UInt64 / Float32 columns present) and holds at least one row.
 Batch arrow_to_protobuf_device(const Processor& proc, Batch& in, cudaStream_t stream) {
+  std::vector<Column*> all;  // the byte extents of a device import's strings (a host import knows them: nothing to launch)
+  for (auto& c : in.cols) all.push_back(&c);
+  resolve_varlen_extents_many(all, stream);
   const auto& ap = static_cast<const ArrowToProtobufProcessor&>(proc);
   const std::vector<PbField>& fields = ap.msg.fields;
   const int64_t n = in.num_rows;

@@ -1,7 +1,7 @@
 // synth.cu — synthetic batches of schema S generated directly in HBM (bench/test support).
 // Twin of oracle/synth.py (same splitmix64 counter RNG), so host and device inputs are identical.
 // Schema S: examples/generate_example.yaml:6 and examples/stream_data.json:1-21 of the reference.
-#include "engine.h"
+#include "abi.h"
 
 namespace ark {
 
@@ -67,14 +67,10 @@ Batch synth_batch(int64_t n, int64_t row0, uint64_t seed, int value_kind, int64_
 
 extern "C" int ark_synth_batch_device(int64_t n_rows, int64_t row0, uint64_t seed, int value_kind, int64_t key_space,
                                       ArrowDeviceArray* out, ArrowSchema* out_schema) {
-  try {
+  return ark::guarded([&] {
+    ark::zero_out(out, out_schema);
     ark::StreamLease lease;
     ark::Batch b = ark::synth_batch(n_rows, row0, seed, value_kind, key_space, lease.s);
-    ARK_CUDA(cudaStreamSynchronize(lease.s));
-    ark::export_device(b, out, out_schema);
-    return ARK_OK;
-  } catch (const ark::ArkError& e) {
-    ark::set_last_error(e.what());
-    return e.code;
-  }
+    ark::export_device(b, out, out_schema, lease);
+  });
 }
