@@ -43,6 +43,18 @@ __global__ void realign_bits_kernel(const uint8_t* in, uint8_t* out, int64_t n, 
   out[byte] = (uint8_t)v;
 }
 
+// zero bits of `bits` over [bit0, bit0 + n), 32 bits per thread
+__global__ void count_zeros_kernel(const uint8_t* bits, int64_t bit0, int64_t n, unsigned long long* zeros) {
+  const int64_t i0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * 32;
+  int z = 0;
+  for (int64_t i = i0; i < n && i < i0 + 32; ++i) {
+    const int64_t b = bit0 + i;
+    z += ((bits[b >> 3] >> (b & 7)) & 1) ^ 1;
+  }
+  z = (int)warp_sum(z);
+  if ((threadIdx.x & 31) == 0 && z) atomicAdd(zeros, (unsigned long long)z);
+}
+
 }  // namespace
 
 BufferPtr pack_bits(const uint8_t* bytes, int64_t n, unsigned long long* zeros, cudaStream_t stream) {
@@ -81,6 +93,12 @@ void set_validity_unknown(Column& c, const BufferPtr& bytes, int64_t n, cudaStre
   if (n == 0) { set_validity(c, nullptr, 0); return; }
   set_validity(c, pack_bits((const uint8_t*)bytes.get(), n, nullptr, stream), -1);
   c.owners.push_back(bytes);
+}
+
+void count_zeros(const uint8_t* bits, int32_t bit0, int64_t n, unsigned long long* zeros, cudaStream_t stream) {
+  if (n <= 0) return;
+  KernelTimer t("count_zeros_kernel", stream);
+  count_zeros_kernel<<<(unsigned)ceil_div(ceil_div(n, 32), 256), 256, 0, stream>>>(bits, bit0, n, zeros);
 }
 
 BufferPtr realign_bits(const uint8_t* in, int32_t bit0, int64_t n, cudaStream_t stream) {

@@ -34,6 +34,10 @@ void set_validity_exact(Column& c, const uint8_t* bytes, int64_t n, cudaStream_t
 // c's validity from bytes[0 .. n) with null_count -1, attached when n > 0 and kept alive with `bytes`.
 void set_validity_unknown(Column& c, const BufferPtr& bytes, int64_t n, cudaStream_t stream);
 
+// Adds the number of zero bits among the n bits of `bits` from bit `bit0` on to the device counter `zeros`: the null count
+// of a validity bitmap that a column shares with a larger one (a slice).
+void count_zeros(const uint8_t* bits, int32_t bit0, int64_t n, unsigned long long* zeros, cudaStream_t stream);
+
 // The n bits of `in` from bit `bit0` on, copied into a fresh bitmap of (n + 7) / 8 bytes that starts at bit 0.  n > 0.
 BufferPtr realign_bits(const uint8_t* in, int32_t bit0, int64_t n, cudaStream_t stream);
 

@@ -7,13 +7,15 @@
 //               immutable, so here the replicated payload column is built ONCE in HBM (replicate kernel) and every
 //               read() hands out another reference to it — BASELINE configs[4]'s "100 M msg/s generate input" costs
 //               no memory traffic at all until a processor reads the messages.
-//   file      ← crates/arkflow-plugin/src/input/file.rs:395-455 (`input_type: {type: json | csv | avro, path}`,
+//   file      ← crates/arkflow-plugin/src/input/file.rs:395-455 (`input_type: {type: json | csv | avro | arrow, path}`,
 //               optional `query`): the file's bytes go to HBM once; line starts are found by a newline-index kernel,
 //               NDJSON lines are decoded by the json_to_arrow kernels (csrc/json.cu), CSV rows by csv_parse_kernel,
 //               Avro object container files (codecs null and snappy) by the kernels of csrc/avro.cu, whose block table
-//               is built on the host while the upload's chunks pass; the optional query runs through the sql
-//               processor.  Parquet / Arrow IPC, the Avro codecs deflate / zstandard / bzip2 / xz and remote object
-//               stores are not read here (ARK_ERR_UNSUPPORTED).
+//               is built on the host while the upload's chunks pass, Arrow IPC files (uncompressed and LZ4_FRAME
+//               bodies) by csrc/arrow_ipc.cu, whose metadata is read before the upload and whose batches are views of
+//               the uploaded file where they can be; the optional query runs through the sql processor.  Parquet, ZSTD
+//               IPC bodies, the Avro codecs deflate / zstandard / bzip2 / xz and remote object stores are not read here
+//               (ARK_ERR_UNSUPPORTED).
 //               The NDJSON schema is merged over the first 1000 records and fixed for the file, as DataFusion does.
 //               Deviations from DataFusion's readers: CSV types come from the first 1000 records with the
 //               types Int64 / Float64 / Boolean / Utf8 (dates stay strings), quoted CSV fields may not contain line
@@ -257,7 +259,7 @@ unsigned grid_of(long long n, int threads = 256) { return (unsigned)std::max<lon
 }  // namespace
 
 struct ark_input {
-  enum Kind { Generate, FileJson, FileCsv, FileAvro } kind = Generate;
+  enum Kind { Generate, FileJson, FileCsv, FileAvro, FileArrow } kind = Generate;
   std::mutex mu;
   // generate
   std::string context;
@@ -282,6 +284,8 @@ struct ark_input {
   bool has_header = true;
   // avro
   std::shared_ptr<AvroFile> avro;  // header, schema and block table
+  // arrow
+  std::shared_ptr<IpcFile> ipc;    // schema and every record batch's nodes and buffers
 };
 
 namespace {
@@ -352,7 +356,7 @@ void file_connect(ark_input* in, cudaStream_t stream, const ChunkVisitor* visit 
   if (io_error) fail(ARK_ERR_PROCESS, "Read input failed: short read on " + in->path);
   if (visit_error) std::rethrow_exception(visit_error);
   in->file_bytes = n;
-  if (in->kind == ark_input::FileAvro) return;  // records are found per batch by avro_index_kernel
+  if (in->kind == ark_input::FileAvro || in->kind == ark_input::FileArrow) return;  // no lines: records come from the block tables
   // line starts
   if (n == 0) { in->n_lines = 0; return; }
   BufferPtr flags = device_alloc((size_t)n);
@@ -595,6 +599,8 @@ bool input_next(ark_input* in, Batch& out, cudaStream_t stream) {
     Batch b;
     if (in->kind == ark_input::FileAvro) {
       b = avro_batch(*in->avro, in->file_dev, l0, n, stream);
+    } else if (in->kind == ark_input::FileArrow) {
+      b = ipc_batch(*in->ipc, in->file_dev, l0, n, stream);
     } else if (in->kind == ark_input::FileJson) {
       BufferPtr h = pinned_alloc(32);
       ARK_CUDA(cudaMemcpyAsync(h.get(), (const long long*)in->line_off.get() + l0, 8, cudaMemcpyDeviceToHost, stream));
@@ -608,7 +614,14 @@ bool input_next(ark_input* in, Batch& out, cudaStream_t stream) {
     if (b.num_rows == 0) continue;  // NDJSON lines that hold only spaces
     if (in->sql) {
       std::vector<Field> fields;
-      for (auto& c : b.cols) { Field f = c.field; if (f.format.empty()) f.format = dtype_arrow_format(f.type); fields.push_back(f); }
+      for (auto& c : b.cols) {
+        Field f = c.field;
+        if (f.format.empty()) f.format = dtype_arrow_format(f.type);
+        // Arrow IPC columns of the types the SQL subset does not compute on (Int32, UInt32, UInt64, Float32) reach the
+        // planner as the sql processor's import presents them, so a query that reads one is Unsupported as it is there
+        if (in->kind == ark_input::FileArrow && fixed_width(f.type) && f.type != DType::Int64 && f.type != DType::Float64) f.type = DType::Null;
+        fields.push_back(f);
+      }
       for (auto& c : b.cols) if (c.field.format.empty()) c.field.format = dtype_arrow_format(c.field.type);
       auto plan = in->sql->plan_for(fields);
       b = in->sql->execute(*plan, b, stream);
@@ -663,8 +676,9 @@ int ark_input_create(const char* type, const char* config_json, ark_input_t** ou
       if (ty->str == "json") in->kind = ark_input::FileJson;
       else if (ty->str == "csv") in->kind = ark_input::FileCsv;
       else if (ty->str == "avro") in->kind = ark_input::FileAvro;
-      else if (ty->str == "parquet" || ty->str == "arrow")
-        fail(ARK_ERR_UNSUPPORTED, "file input: " + ty->str + " files are not decoded on the GPU (json, csv and avro are)");
+      else if (ty->str == "arrow") in->kind = ark_input::FileArrow;
+      else if (ty->str == "parquet")
+        fail(ARK_ERR_UNSUPPORTED, "file input: " + ty->str + " files are not decoded on the GPU (json, csv, avro and arrow are)");
       else fail(ARK_ERR_SERIALIZATION, "unknown variant `" + ty->str + "`, expected one of `avro`, `arrow`, `json`, `csv`, `parquet`");
       const JsonValue* p = it->get("path");
       if (!p || p->kind != JsonValue::String) fail(ARK_ERR_SERIALIZATION, "missing field `path`");
@@ -709,6 +723,18 @@ int ark_input_connect(ark_input_t* in) {
       avro_scan_end(*av);
       in->avro = av;
       in->n_lines = avro_rows(*av);
+      in->next_line = 0;
+      in->connected = true;
+      return;
+    }
+    if (in->kind == ark_input::FileArrow) {
+      // every piece of metadata first (its errors need no device), then the upload
+      std::shared_ptr<IpcFile> ipc = ipc_open(in->path);
+      StreamLease lease;
+      file_connect(in, lease.s);
+      if (!ipc) fail(ARK_ERR_PROCESS, "Read input failed: cannot open " + in->path);
+      in->ipc = ipc;
+      in->n_lines = ipc_rows(*ipc);
       in->next_line = 0;
       in->connected = true;
       return;

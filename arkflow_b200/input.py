@@ -2,7 +2,7 @@
 
     trait Input { connect, read, close }   → class Input          (core/input/mod.rs)
     GenerateInput                          → class GenerateInput  (plugin/input/generate.rs:26-96)
-    FileInput (json / csv / avro)          → class FileInput      (plugin/input/file.rs:395-455)
+    FileInput (json / csv / avro / arrow)  → class FileInput      (plugin/input/file.rs:395-455)
     InputConfig::build                     → build_input(cfg)
 
 read() returns (MessageBatch, NoopAck) like the reference; read_device() leaves the batch in HBM.  End of input is
@@ -63,13 +63,23 @@ class GenerateInput(Input):
 
 
 class FileInput(Input):
-    """`type: file` {input_type: {type: json | csv | avro, path}, query?: {query, table?}, batch_size?}.
+    """`type: file` {input_type: {type: json | csv | avro | arrow, path}, query?: {query, table?}, batch_size?}.
 
     `avro`: object container files with codec null or snappy, decoded on the GPU.  The top-level record's fields may be
     null, boolean, int, long, float, double, bytes or string, or a [null, T] / [T, null] union of one of these: Arrow
     Null, Boolean, Int32, Int64, Float32, Float64, Binary, Utf8, nullable only for unions.  Other schemas and codecs
     raise Unsupported from connect(); malformed data raises Process naming the first failing record and its block's
     file offset (structural damage already from connect()).  SQL `query` over Int32 / Float32 columns is Unsupported.
+
+    `arrow`: Arrow IPC files (the footer-indexed file format, current or pre-0.15 message prefixes) with uncompressed or
+    LZ4_FRAME bodies, read on the GPU.  Fields may be Null, Boolean, Int32, Int64, UInt32, UInt64, Float32, Float64,
+    Utf8 or Binary, nullable or not; every other type (dictionary-encoded, nested, Large / View, Int8 / Int16, temporal,
+    decimal), a big-endian schema and a ZSTD body raise Unsupported from connect(), which reads all metadata before the
+    device is touched.  Structural damage (magic, footer, ranges, sizes, NULLs in a non-nullable field) raises Process
+    from connect(); bad body bytes (LZ4 frames, offsets, UTF-8, a null count that differs from its bitmap) fail the
+    read that first touches the record batch, naming the batch, column and row.  Batches cut through record batches;
+    one that lies inside a single record batch is a view of the file in HBM.  A `query` that reads an Int32, UInt32,
+    UInt64 or Float32 column raises Unsupported, as the sql processor does.  Parquet raises Unsupported.
     """
 
     TYPE = "file"

@@ -319,13 +319,17 @@ int ark_sql_group_by_merge_device(ark_proc_t* p, ark_dist_t* d, struct ArrowDevi
  *        but the first, and returns ARK_ERR_EOF once `count` is reached or the next batch would exceed it.
  *        NULL config → ARK_ERR_CONFIG "Generate input configuration is missing" (generate.rs:107-111).
  *      type "file" ← `impl Input for FileInput`, crates/arkflow-plugin/src/input/file.rs:395-455: config
- *        {input_type: {type: "json" | "csv" | "avro", path}, query?: {query, table?}, batch_size?}; connect() loads the
- *        file into HBM and indexes its lines (Avro: its blocks, from the header and block headers read on the host),
+ *        {input_type: {type: "json" | "csv" | "avro" | "arrow", path}, query?: {query, table?}, batch_size?}; connect()
+ *        loads the file into HBM and indexes its lines (Avro: its blocks, from the header and block headers read on the
+ *        host; Arrow IPC: every record batch's nodes and buffers, from the footer and messages read on the host),
  *        read() decodes the next batch_size lines / records (NDJSON: json_to_arrow kernels; CSV: header + type
  *        inference over the first 1000 rows on the host, csv_parse_kernel; Avro object container files with codec null
  *        or snappy and a record of null / boolean / int / long / float / double / bytes / string fields or [null, T]
- *        unions: csrc/avro.cu) and applies the optional query; ARK_ERR_EOF at the end.  parquet / arrow, other Avro
- *        schemas and codecs (decided by connect()) and remote stores → ARK_ERR_UNSUPPORTED.
+ *        unions: csrc/avro.cu; Arrow IPC files, uncompressed or LZ4_FRAME bodies, of Null / Boolean / Int32 / Int64 /
+ *        UInt32 / UInt64 / Float32 / Float64 / Utf8 / Binary fields: csrc/arrow_ipc.cu, validated on the device, a
+ *        batch inside one stored batch is a view of the uploaded file) and applies the optional query; ARK_ERR_EOF at
+ *        the end.  parquet, other Avro schemas and codecs, other Arrow types, big-endian schemas and ZSTD bodies
+ *        (decided by connect()) and remote stores → ARK_ERR_UNSUPPORTED.
  *      ark_input_read_device leaves the batch in HBM (feed it to ark_buffer_write_device / *_process_device). ---- */
 int ark_input_create(const char* type, const char* config_json, ark_input_t** out);
 int ark_input_connect(ark_input_t* in);
