@@ -7,7 +7,7 @@
 // (continuation-marker or legacy pre-0.15 length prefix), its field nodes and buffers and, in a compressed body, the
 // 8-byte uncompressed-length prefix of every buffer.  The flatbuffers are read by the bounds-checked reader below.  Every
 // buffer's range, node length and (uncompressed) size is checked against the body, the file and what its type needs.
-// The file's bytes then go to HBM once (inputs.cu's file_connect).
+// The file's bytes then go to HBM once (the file driver's upload).
 //
 // A read of rows [r0, r0 + n) decodes every stored record batch it touches for the first time, as a whole, and keeps
 // the last one when it reaches into the next read:
@@ -26,17 +26,13 @@
 // Errors are Process "Read input failed: Arrow IPC error: <what> (record batch k[, column 'c'][, row r])": a check that
 // needs only metadata and length prefixes fails connect(), one that needs body bytes fails the read of the batch.
 // oracle/arrow_ipc_oracle.py restates all of this in Python; tests/test_arrow_ipc_input_gpu.py compares the two.
-#include <fcntl.h>
-#include <sys/stat.h>
-#include <unistd.h>
-
 #include <algorithm>
 #include <array>
 #include <climits>
 #include <cstring>
 
 #include "bitmap.h"
-#include "engine.h"
+#include "file_input.h"
 #include "utf8.cuh"
 #include "varlen.h"
 
@@ -256,26 +252,10 @@ bool field_type(const FbTable& f, DType* out, std::string* desc) {
   return ok;
 }
 
-struct Fd {
-  int fd;
-  int64_t size;
-  ~Fd() { if (fd >= 0) close(fd); }
-  std::string read(int64_t off, int64_t n) const {
-    std::string s((size_t)n, '\0');
-    int64_t done = 0;
-    while (done < n) {
-      const ssize_t got = pread(fd, &s[(size_t)done], (size_t)(n - done), (off_t)(off + done));
-      if (got <= 0) fail(ARK_ERR_PROCESS, "Read input failed: short read");
-      done += got;
-    }
-    return s;
-  }
-};
-
 int64_t le64(const std::string& s, size_t at) { int64_t v; memcpy(&v, s.data() + at, 8); return v; }
 int32_t le32(const std::string& s, size_t at) { int32_t v; memcpy(&v, s.data() + at, 4); return v; }
 
-void read_batch_meta(IpcFile& f, const Fd& fd, size_t k, int64_t off, int64_t meta_len, int64_t body_len, int64_t end) {
+void read_batch_meta(IpcFile& f, const HostFile& fd, size_t k, int64_t off, int64_t meta_len, int64_t body_len, int64_t end) {
   IpcStored S;
   S.offset = off;
   const std::string kb = at_batch(k);
@@ -354,14 +334,7 @@ void read_batch_meta(IpcFile& f, const Fd& fd, size_t k, int64_t off, int64_t me
   f.batches.push_back(std::move(S));
 }
 
-}  // namespace
-
-std::shared_ptr<IpcFile> ipc_open(const std::string& path) {
-  Fd fd{open(path.c_str(), O_RDONLY), 0};
-  if (fd.fd < 0) return nullptr;  // file_connect reports it
-  struct stat st;
-  if (fstat(fd.fd, &st) != 0) return nullptr;
-  fd.size = (int64_t)st.st_size;
+void ipc_open(IpcFile& f, const HostFile& fd) {
   const int64_t n = fd.size;
   if (n < 18 || fd.read(0, 6) != "ARROW1" || fd.read(n - 6, 6) != "ARROW1") ipc_fail("not an Arrow IPC file (bad magic)");
   const int64_t flen = le32(fd.read(n - 10, 4), 0);
@@ -369,7 +342,6 @@ std::shared_ptr<IpcFile> ipc_open(const std::string& path) {
   const int64_t foot = n - 10 - flen;
   const std::string fbytes = fd.read(foot, flen);
   const Fb fb{(const uint8_t*)fbytes.data(), fbytes.size()};
-  auto f = std::make_shared<IpcFile>();
   struct Block { int64_t off, meta, body; };
   std::vector<Block> blocks;
   try {
@@ -386,7 +358,7 @@ std::shared_ptr<IpcFile> ipc_open(const std::string& path) {
       F.nullable = fl.scalar<uint8_t>(1, 0) != 0;
       std::string desc;
       if (!field_type(fl, &F.type, &desc)) fail(ARK_ERR_UNSUPPORTED, "arrow input: field '" + F.name + "' has type " + desc + ", which is not decoded on the GPU");
-      f->fields.push_back(F);
+      f.fields.push_back(F);
     }
     const auto rbs = footer.vec(3, 24);
     for (size_t k = 0; k < rbs.second; ++k)
@@ -394,11 +366,11 @@ std::shared_ptr<IpcFile> ipc_open(const std::string& path) {
   } catch (const FbError&) {
     ipc_fail("malformed footer");
   }
-  for (size_t k = 0; k < blocks.size(); ++k) read_batch_meta(*f, fd, k, blocks[k].off, blocks[k].meta, blocks[k].body, foot);
-  return f;
+  for (size_t k = 0; k < blocks.size(); ++k) read_batch_meta(f, fd, k, blocks[k].off, blocks[k].meta, blocks[k].body, foot);
 }
 
-int64_t ipc_rows(const IpcFile& f) { return f.rows; }
+}  // namespace
+
 
 namespace {
 
@@ -760,5 +732,27 @@ Batch ipc_batch(IpcFile& f, const BufferPtr& file_dev, int64_t r0, int64_t n, cu
   }
   return out;
 }
+
+namespace {
+
+struct IpcFormat : FileFormat {
+  IpcFile f;
+  BufferPtr file_dev;
+
+  // every piece of metadata, whose errors need no device
+  void open(const HostFile& file) override {
+    f = IpcFile();
+    ipc_open(f, file);
+  }
+  int64_t prepare(const BufferPtr& dev, int64_t, cudaStream_t) override {
+    file_dev = dev;
+    return f.rows;
+  }
+  Batch batch(int64_t r0, int64_t n, cudaStream_t stream) override { return ipc_batch(f, file_dev, r0, n, stream); }
+};
+
+}  // namespace
+
+std::unique_ptr<FileFormat> make_arrow_ipc_format() { return std::make_unique<IpcFormat>(); }
 
 }  // namespace ark

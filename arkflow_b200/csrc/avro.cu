@@ -1,6 +1,6 @@
 // avro.cu — the `file` input's `avro` type: Avro object container files (spec 1.11) decoded on the device.
 //
-// The file's bytes go to HBM once (inputs.cu's file_connect); on the host, while the chunks stream past, AvroScan walks
+// The file's bytes go to HBM once (the file driver's upload); on the host, while the chunks stream past, avro_scan walks
 // the header and every block header and builds the block table {data offset, size, count, first row, uncompressed
 // length}.  A batch of rows [r0, r0 + n) then runs:
 //   avro_snappy_kernel  (codec snappy) one warp per block of the batch decompresses into an arena laid out by a host scan
@@ -33,7 +33,7 @@
 #include <cstdio>
 
 #include "bitmap.h"
-#include "engine.h"
+#include "file_input.h"
 #include "json_mini.h"
 #include "tma.cuh"
 #include "utf8.cuh"
@@ -234,28 +234,6 @@ int64_t parse_header(AvroFile& f, const std::string& h, bool eof) {
   return (int64_t)q;
 }
 
-}  // namespace
-
-std::shared_ptr<AvroFile> avro_open(const std::string& path) {
-  FILE* fp = fopen(path.c_str(), "rb");
-  if (!fp) return nullptr;  // file_connect reports it
-  auto f = std::make_shared<AvroFile>();
-  std::string h;
-  char buf[1 << 16];
-  int64_t len = 0;
-  while (true) {
-    const size_t got = fread(buf, 1, sizeof buf, fp);
-    h.append(buf, got);
-    const bool eof = got < sizeof buf;
-    try { len = parse_header(*f, h, eof); } catch (...) { fclose(fp); throw; }
-    if (len > 0) break;
-  }
-  fclose(fp);
-  f->header_bytes = len;
-  f->pos = len;
-  return f;
-}
-
 // The file's bytes [base, base + n), in order, after the header.  Block headers and sync markers may straddle two calls.
 void avro_scan(AvroFile& f, const uint8_t* p, size_t n, int64_t base) {
   const int64_t end = base + (int64_t)n;
@@ -321,10 +299,6 @@ void avro_scan_end(AvroFile& f) {
   const int64_t off = f.state == AvroFile::BlockHeader ? f.pos : f.blocks[(size_t)f.cur].offset;
   av_fail("truncated block (block at offset " + std::to_string(off) + ")");
 }
-
-int64_t avro_rows(const AvroFile& f) { return f.rows; }
-
-namespace {
 
 // ---- device --------------------------------------------------------------------------------------------------------
 struct AvBlockDev {
@@ -609,8 +583,6 @@ __global__ void __launch_bounds__(AV_THREADS) avro_decode_kernel(const __grid_co
   if (!av_record<true>(P, p, end, origin, i, err)) atomicMin(P.error, ((unsigned long long)(P.row0 + i) << 8) | (unsigned)err);
 }
 
-}  // namespace
-
 Batch avro_batch(AvroFile& f, const BufferPtr& file_dev, int64_t r0, int64_t n, cudaStream_t stream) {
   // the blocks that hold rows [r0, r0 + n): the first whose rows reach past r0, up to the first that starts at r0 + n
   auto by_row = [](const AvroBlock& b, int64_t r) { return b.first_row + b.count <= r; };
@@ -741,5 +713,35 @@ Batch avro_batch(AvroFile& f, const BufferPtr& file_dev, int64_t r0, int64_t n, 
   ARK_CUDA(cudaStreamSynchronize(stream));
   return out;
 }
+
+struct AvroFormat : FileFormat {
+  AvroFile f;
+  BufferPtr file_dev;
+
+  // the header (schema and codec), whose errors need no device
+  void open(const HostFile& file) override {
+    f = AvroFile();
+    std::string h;
+    char buf[1 << 16];
+    while (true) {
+      const size_t got = file.read_some((int64_t)h.size(), buf, sizeof buf);
+      h.append(buf, got);
+      const int64_t len = parse_header(f, h, got < sizeof buf);
+      if (len > 0) { f.header_bytes = len; f.pos = len; return; }
+    }
+  }
+  // the block table, built while the upload's chunks pass
+  void scan(const uint8_t* p, size_t n, int64_t base) override { avro_scan(f, p, n, base); }
+  int64_t prepare(const BufferPtr& dev, int64_t, cudaStream_t) override {
+    avro_scan_end(f);
+    file_dev = dev;
+    return f.rows;
+  }
+  Batch batch(int64_t r0, int64_t n, cudaStream_t stream) override { return avro_batch(f, file_dev, r0, n, stream); }
+};
+
+}  // namespace
+
+std::unique_ptr<FileFormat> make_avro_format() { return std::make_unique<AvroFormat>(); }
 
 }  // namespace ark

@@ -97,18 +97,6 @@ const std::string& protobuf_to_arrow_value_field(const Processor& p);
 Batch protobuf_to_arrow_device(const Processor& proc, Batch& in, cudaStream_t stream);
 std::unique_ptr<Processor> make_arrow_to_protobuf(const char* config_json);
 Batch arrow_to_protobuf_device(const Processor& proc, Batch& in, cudaStream_t stream);
-// avro.cu: the `file` input's Avro object container files
-struct AvroFile;
-std::shared_ptr<AvroFile> avro_open(const std::string& path);  // header, schema and codec (nullptr: cannot open)
-void avro_scan(AvroFile& f, const uint8_t* p, size_t n, int64_t base);  // the block table, from the file's bytes in order
-void avro_scan_end(AvroFile& f);
-int64_t avro_rows(const AvroFile& f);
-Batch avro_batch(AvroFile& f, const BufferPtr& file_dev, int64_t r0, int64_t n, cudaStream_t stream);
-// arrow_ipc.cu: the `file` input's Arrow IPC files
-struct IpcFile;
-std::shared_ptr<IpcFile> ipc_open(const std::string& path);  // every piece of metadata, read with pread (nullptr: cannot open)
-int64_t ipc_rows(const IpcFile& f);
-Batch ipc_batch(IpcFile& f, const BufferPtr& file_dev, int64_t r0, int64_t n, cudaStream_t stream);
 Batch concat_device(std::vector<Batch>& ins, cudaStream_t stream);
 Batch synth_batch(int64_t n, int64_t row0, uint64_t seed, int value_kind, int64_t key_space, cudaStream_t stream);
 

@@ -1,4 +1,4 @@
-"""CPU oracle for the CSV scan of the `file` input (csrc/inputs.cu) — TEST INFRASTRUCTURE (see oracle/__init__.py).
+"""CPU oracle for the CSV scan of the `file` input (csrc/csv.cu) — TEST INFRASTRUCTURE (see oracle/__init__.py).
 
 The reference reads a CSV file with DataFusion's `ctx.read_csv(path, CsvReadOptions::default())`
 (crates/arkflow-plugin/src/input/file.rs:229-237), which is arrow-csv 55.2 over csv-core.  This module restates, in
@@ -18,7 +18,7 @@ plain Python and without pyarrow.csv, the contract the library documents for tha
     number of fields comes first, then a value that does not parse, then invalid UTF-8 in a Utf8 field;
   * more than 32 columns is Unsupported.
 
-Where this contract differs from arrow-csv (csrc/inputs.cu's header names the first three):
+Where this contract differs from arrow-csv (csrc/csv.cu's header names the first three):
   * quoted fields may not contain line breaks: a line break always ends the record;
   * dates and timestamps stay Utf8 (arrow-csv infers Date32 / Timestamp);
   * the sample is the first 1000 records as here, but arrow-csv's integer pattern has no leading `+`: `+5` is Utf8
