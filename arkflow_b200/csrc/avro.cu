@@ -11,8 +11,8 @@
 //   avro_decode_kernel  one thread per record (the records of a CTA arrive in shared memory by one 1-D TMA bulk copy):
 //                       fixed-width values and validity go to their rows, string / bytes record their spans, and strings
 //                       are checked for UTF-8 in the same pass;
-//   strings             exclusive scan of the span lengths behind the 2 GiB int32-offset guard, then a span copy
-//                       (varlen.cu's varlen_guard / varlen_scan / launch_span_copy).
+//   columns             settled and built by decoded.h (the error word before the 2 GiB guard; scans, validity and null
+//                       counts in one round trip), string bytes by a span copy (varlen.h's launch_span_copy).
 // Schema: a record whose fields are null, boolean, int, long, float, double, bytes or string, or a two-branch union of
 // null and one of these in either order → Null, Boolean, Int32, Int64, Float32, Float64, Binary, Utf8 (DataFusion's Avro
 // reader's mapping); a plain field is non-nullable, a union field nullable.  Anything else (nested record, array, map,
@@ -32,9 +32,10 @@
 #include <algorithm>
 #include <cstdio>
 
-#include "bitmap.h"
+#include "decoded.h"
 #include "file_input.h"
 #include "json_mini.h"
+#include "stage_store.cuh"
 #include "tma.cuh"
 #include "utf8.cuh"
 #include "varlen.h"
@@ -621,92 +622,47 @@ Batch avro_batch(AvroFile& f, const BufferPtr& file_dev, int64_t r0, int64_t n, 
   ARK_CUDA(cudaMemsetAsync(err.get(), 0xFF, 8, stream));
   ARK_CUDA(cudaMemsetAsync(rs.get(), 0xFF, (size_t)n * 8, stream));  // unlocated until avro_index_kernel finds it
   P.rec_start = (const long long*)rs.get(); P.rec_end = (const long long*)re.get(); P.error = (unsigned long long*)err.get();
-  std::vector<BufferPtr> values(nf), valid(nf), src(nf), lens(nf);
+  // a record's strings lie inside the record, so the bytes the batch's blocks span bound every string column's total
+  int64_t bound = 0;
+  for (auto& d : hb) bound += d.end - d.start;
+  std::vector<StagedColumn> cols;
   for (size_t k = 0; k < nf; ++k) {
     const AvroField& a = f.fields[k];
+    cols.push_back(stage_column(av_dtype(a.kind), n, a.null_branch >= 0, false, stream));
+    StagedColumn& s = cols.back();
+    s.bound = bound; s.what = "avro input: column '" + a.name + "'";
     AvField& F = P.f[k];
     F.kind = a.kind; F.null_branch = a.null_branch;
-    if (a.null_branch >= 0) { valid[k] = device_alloc((size_t)n); F.valid = (uint8_t*)valid[k].get(); }
-    if (a.kind == AK_BYTES || a.kind == AK_STRING) {
-      src[k] = device_alloc((size_t)n * 8); lens[k] = device_alloc((size_t)(n + 1) * 4);
-      ARK_CUDA(cudaMemsetAsync(lens[k].get(), 0, (size_t)(n + 1) * 4, stream));  // a failed batch may leave rows unwritten
-      F.str_src = (long long*)src[k].get(); F.str_len = (int32_t*)lens[k].get();
-    } else if (a.kind != AK_NULL) {
-      F.width = a.kind == AK_BOOL ? 1 : (uint8_t)fixed_width(av_dtype(a.kind));
-      values[k] = device_alloc((size_t)n * F.width);
-      F.values = values[k].get();
-    }
+    F.values = s.values.get(); F.valid = (uint8_t*)s.valid.get(); F.str_src = (long long*)s.src.get(); F.str_len = (int32_t*)s.len.get();
+    if (s.values) F.width = a.kind == AK_BOOL ? 1 : (uint8_t)fixed_width(s.type);
   }
   {
     KernelTimer t("avro_index_kernel", stream);
     avro_index_kernel<<<(unsigned)ceil_div(nb, 128), 128, 0, stream>>>(P, (const AvBlockDev*)dblk.get(), nb, (const int32_t*)status.get(), (long long*)rs.get(), (long long*)re.get());
   }
   {
-    // staging window: the CTA's record bytes + slack; records that average more than 256 bytes are parsed in place
-    const int64_t span = hb.empty() ? 0 : hb.back().end - hb.front().start;
-    const double avg = (double)span / (double)n;
-    P.stage_bytes = avg <= 256.0 ? (int)round_up((int64_t)(avg * AV_THREADS * 1.25) + 256, 1024) : 0;
+    P.stage_bytes = record_stage_window(hb.empty() ? 0 : hb.back().end - hb.front().start, n, AV_THREADS);
     KernelTimer t("avro_decode_kernel", stream);
     avro_decode_kernel<<<(unsigned)ceil_div(n, AV_THREADS), AV_THREADS, (size_t)P.stage_bytes + 32, stream>>>(P);
   }
   ARK_CUDA(cudaGetLastError());
-  // a record's strings lie inside the record, so the bytes the batch's blocks span bound every string column's total
-  int64_t bound = 0;
-  for (auto& d : hb) bound += d.end - d.start;
-  BufferPtr h = pinned_alloc(8 + 16 * nf);
-  auto error_check = [&]() {
-    const unsigned long long e = *(const unsigned long long*)h.get();
+  settle_columns(cols, err.get(), 8, [&](const void* h) {
+    const unsigned long long e = *(const unsigned long long*)h;
     if (e == ~0ull) return;
     const int64_t row = (int64_t)(e >> 8);
     auto it = std::lower_bound(f.blocks.begin(), f.blocks.end(), row, by_row);
     av_fail(std::string(av_err_text((int)(e & 0xFF))) + " in record " + std::to_string(row) + " (block at offset " + std::to_string(it->offset) + ")");
-  };
-  if (bound > INT32_MAX) {  // the error decides before the 2 GiB guard reads the lengths
-    ARK_CUDA(cudaMemcpyAsync(h.get(), err.get(), 8, cudaMemcpyDeviceToHost, stream));
-    ARK_CUDA(cudaStreamSynchronize(stream));
-    error_check();
-    for (size_t k = 0; k < nf; ++k)
-      if (lens[k]) varlen_guard((const int32_t*)lens[k].get(), n, bound, "avro input: column '" + f.fields[k].name + "'", stream);
-  }
-  // the error word, every string total and every null count come back in one round trip
-  std::vector<BufferPtr> offs(nf), vbits(nf);
-  BufferPtr zeros = device_alloc(8 * std::max<size_t>(nf, 1));
-  ARK_CUDA(cudaMemsetAsync(zeros.get(), 0, 8 * std::max<size_t>(nf, 1), stream));
-  ARK_CUDA(cudaMemcpyAsync(h.get(), err.get(), 8, cudaMemcpyDeviceToHost, stream));
-  for (size_t k = 0; k < nf; ++k) {
-    if (lens[k]) {
-      offs[k] = varlen_scan((const int32_t*)lens[k].get(), n, stream);
-      ARK_CUDA(cudaMemcpyAsync((char*)h.get() + 8 + 16 * k, (int32_t*)offs[k].get() + n, 4, cudaMemcpyDeviceToHost, stream));
-    }
-    if (valid[k]) {
-      vbits[k] = pack_bits((const uint8_t*)valid[k].get(), n, (unsigned long long*)zeros.get() + k, stream);
-      ARK_CUDA(cudaMemcpyAsync((char*)h.get() + 16 + 16 * k, (unsigned long long*)zeros.get() + k, 8, cudaMemcpyDeviceToHost, stream));
-    }
-  }
-  ARK_CUDA(cudaStreamSynchronize(stream));
-  error_check();
+  }, stream);
 
   Batch out;
   out.num_rows = n;
   for (size_t k = 0; k < nf; ++k) {
     const AvroField& a = f.fields[k];
     const DType t = av_dtype(a.kind);
-    Column c;
-    c.field.name = a.name; c.field.type = t; c.field.format = dtype_arrow_format(t);
-    c.field.nullable = a.null_branch >= 0 || a.kind == AK_NULL;
-    c.length = n;
-    if (a.kind == AK_NULL) { c.null_count = n; out.cols.push_back(std::move(c)); continue; }
-    if (offs[k]) {
-      const int32_t total = *(const int32_t*)((char*)h.get() + 8 + 16 * k);
-      BufferPtr bytes = device_alloc((size_t)total + 16);
-      if (total) launch_span_copy(P.arena, nullptr, (const long long*)src[k].get(), (const int32_t*)offs[k].get(), n, (uint8_t*)bytes.get(), stream);
-      set_varlen(c, {offs[k], bytes, total});
-    } else if (t == DType::Bool) {
-      set_bool_values(c, values[k], n, stream);
-    } else {
-      c.data = (const uint8_t*)values[k].get(); c.data_bytes = n * fixed_width(t); c.owners = {values[k]};
-    }
-    set_validity(c, vbits[k], valid[k] ? *(const long long*)((char*)h.get() + 16 + 16 * k) : 0);
+    Column c = finish_column(cols[k], Field{a.name, t, a.null_branch >= 0 || a.kind == AK_NULL, dtype_arrow_format(t)}, [&](const StagedColumn& s, uint8_t* bytes) {
+      if (s.total) launch_span_copy(P.arena, nullptr, (const long long*)s.src.get(), (const int32_t*)s.offsets.get(), n, bytes, stream);
+    }, stream);
+    if (a.kind == AK_NULL) c.null_count = n;
     out.cols.push_back(std::move(c));
   }
   ARK_CUDA(cudaGetLastError());

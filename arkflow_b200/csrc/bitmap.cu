@@ -79,16 +79,6 @@ void set_validity(Column& c, const BufferPtr& bits, int64_t null_count) {
   c.owners.push_back(bits);
 }
 
-void set_validity_exact(Column& c, const uint8_t* bytes, int64_t n, cudaStream_t stream) {
-  if (n == 0) { set_validity(c, nullptr, 0); return; }
-  BufferPtr zeros = device_alloc(8), h = pinned_alloc(8);
-  ARK_CUDA(cudaMemsetAsync(zeros.get(), 0, 8, stream));
-  BufferPtr bits = pack_bits(bytes, n, (unsigned long long*)zeros.get(), stream);
-  ARK_CUDA(cudaMemcpyAsync(h.get(), zeros.get(), 8, cudaMemcpyDeviceToHost, stream));
-  ARK_CUDA(cudaStreamSynchronize(stream));
-  set_validity(c, bits, *(const long long*)h.get());
-}
-
 void set_validity_unknown(Column& c, const BufferPtr& bytes, int64_t n, cudaStream_t stream) {
   if (n == 0) { set_validity(c, nullptr, 0); return; }
   set_validity(c, pack_bits((const uint8_t*)bytes.get(), n, nullptr, stream), -1);

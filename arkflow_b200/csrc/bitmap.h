@@ -6,10 +6,8 @@
 //
 // A column's null_count is exact or -1 (unknown), and a column whose count is 0 carries no validity bitmap.  Which of
 // the two a producer gives depends on what the count costs it:
-//   * exact: the inputs and decoders (CSV, JSON, Avro) count the zero bytes while packing and read the count back.
-//     A single-column producer does it in set_validity_exact, one synchronisation per column.  A producer that makes one
-//     round trip for all its columns' totals gives pack_bits a counter slot of that round trip and calls set_validity
-//     after its synchronisation.
+//   * exact: the decoders (CSV, JSON, Avro) count the zero bytes while packing, in a counter slot of the one round trip
+//     that settles all the columns of a batch (decoded.h), and call set_validity after its synchronisation.
 //   * unknown: query outputs (SQL projection, join gathers, GROUP BY keys and aggregates) take no read-back and no
 //     synchronisation; set_validity_unknown attaches the bitmap whenever there are rows.
 #pragma once
@@ -26,10 +24,6 @@ void set_bool_values(Column& c, const BufferPtr& bytes, int64_t n, cudaStream_t 
 
 // Attaches `bits` as c's validity with `null_count` (-1: unknown); a count of 0 attaches nothing.
 void set_validity(Column& c, const BufferPtr& bits, int64_t null_count);
-
-// c's validity from bytes[0 .. n) with its exact null count: one read-back and one synchronisation when n > 0.  `bytes`
-// is not kept.
-void set_validity_exact(Column& c, const uint8_t* bytes, int64_t n, cudaStream_t stream);
 
 // c's validity from bytes[0 .. n) with null_count -1, attached when n > 0 and kept alive with `bytes`.
 void set_validity_unknown(Column& c, const BufferPtr& bytes, int64_t n, cudaStream_t stream);

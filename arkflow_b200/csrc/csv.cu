@@ -11,8 +11,8 @@
 // a closing quote count as such), then a value that does not parse as its column's type (invalid UTF-8 in a numeric or
 // Boolean field is this error), then invalid UTF-8 in a Utf8 field.  tests/test_inputs_edges_gpu.py checks all of this
 // against oracle/csv_oracle.py.
-#include "bitmap.h"
 #include "decimal.cuh"
+#include "decoded.h"
 #include "file_input.h"
 #include "utf8.cuh"
 #include "varlen.h"
@@ -229,65 +229,46 @@ struct CsvFormat : FileFormat {
     const auto [byte0, byte1] = lines.span(l0, n, stream);
     BufferPtr loff = lines.rebased(l0, n, stream);
     P.data = (const uint8_t*)lines.file.get() + byte0; P.line_off = (const int32_t*)loff.get(); P.n_rows = n; P.n_cols = nc; P.delim = delim;
-    std::vector<BufferPtr> vals(nc), valid(nc), slen(nc), ssrc(nc), sraw(nc);
     BufferPtr err = device_alloc(16);
     ARK_CUDA(cudaMemsetAsync(err.get(), 0xFF, 16, stream));
     P.error = (unsigned long long*)err.get();
+    static const DType dtype[] = {DType::Int64, DType::Float64, DType::Bool, DType::Utf8};
+    std::vector<StagedColumn> cols;
     for (int c = 0; c < nc; ++c) {
       P.types[c] = types[c];
-      valid[c] = device_alloc((size_t)std::max<int64_t>(n, 1));
-      P.valid[c] = (uint8_t*)valid[c].get();
-      if (types[c] == CSV_STR) {
-        slen[c] = device_alloc((size_t)(n + 1) * 4); ssrc[c] = device_alloc((size_t)std::max<int64_t>(n, 1) * 8); sraw[c] = device_alloc((size_t)std::max<int64_t>(n, 1) * 4);
-        ARK_CUDA(cudaMemsetAsync((int32_t*)slen[c].get() + n, 0, 4, stream));
-        P.str_len[c] = (int32_t*)slen[c].get(); P.str_src[c] = (long long*)ssrc[c].get(); P.str_raw[c] = (int32_t*)sraw[c].get();
-      } else {
-        vals[c] = device_alloc((size_t)std::max<int64_t>(n, 1) * (types[c] == CSV_BOOL ? 1 : 8));
-        P.values[c] = vals[c].get();
-      }
+      cols.push_back(stage_column(dtype[types[c]], n, true, true, stream));
+      StagedColumn& s = cols.back();
+      P.valid[c] = (uint8_t*)s.valid.get();
+      P.values[c] = s.values.get();
+      P.str_len[c] = (int32_t*)s.len.get(); P.str_src[c] = (long long*)s.src.get(); P.str_raw[c] = (int32_t*)s.raw.get();
+      // a field's bytes lie inside its line, so the batch's byte span (at most 2 GiB, checked above) bounds the column
+      s.bound = byte1 - byte0; s.what = "file input: column '" + names[c] + "'";
     }
     {
       KernelTimer t("csv_parse_kernel", stream);
       csv_parse_kernel<<<grid_of(n, 128), 128, 0, stream>>>(P);
     }
     ARK_CUDA(cudaGetLastError());
-    BufferPtr herr = pinned_alloc(16);
-    ARK_CUDA(cudaMemcpyAsync(herr.get(), err.get(), 8, cudaMemcpyDeviceToHost, stream));
-    ARK_CUDA(cudaStreamSynchronize(stream));
-    const unsigned long long ekey = *(const unsigned long long*)herr.get();
-    if (ekey != ~0ull) {
+    settle_columns(cols, err.get(), 8, [&](const void* h) {
+      const unsigned long long ekey = *(const unsigned long long*)h;
+      if (ekey == ~0ull) return;
       const int ecode = (int)(ekey & 3);
-      ARK_CUDA(cudaMemcpyAsync(herr.get(), (const long long*)lines.starts.get() + l0 + (long long)(ekey >> 2), 8, cudaMemcpyDeviceToHost, stream));
+      BufferPtr hstart = pinned_alloc(8);
+      ARK_CUDA(cudaMemcpyAsync(hstart.get(), (const long long*)lines.starts.get() + l0 + (long long)(ekey >> 2), 8, cudaMemcpyDeviceToHost, stream));
       ARK_CUDA(cudaStreamSynchronize(stream));
-      const long long lineno = lines.physical_line(*(const long long*)herr.get(), stream);
+      const long long lineno = lines.physical_line(*(const long long*)hstart.get(), stream);
       fail(ARK_ERR_PROCESS, ecode == 2 ? "Read input failed: Arrow error: Csv error: incorrect number of fields for line " + std::to_string(lineno)
                             : ecode == 3 ? "Read input failed: Arrow error: Csv error: Encountered invalid UTF-8 data for line " + std::to_string(lineno)
                                          : "Read input failed: Arrow error: Parser error: Error while parsing value of line " + std::to_string(lineno));
-    }
+    }, stream);
     Batch b;
     b.num_rows = n;
-    for (int c = 0; c < nc; ++c) {
-      Column col;
-      col.field.name = names[c]; col.field.nullable = true; col.length = n;
-      switch (types[c]) {
-        case CSV_I64: col.field.type = DType::Int64; col.field.format = "l"; col.data = (const uint8_t*)vals[c].get(); col.data_bytes = n * 8; col.owners = {vals[c]}; break;
-        case CSV_F64: col.field.type = DType::Float64; col.field.format = "g"; col.data = (const uint8_t*)vals[c].get(); col.data_bytes = n * 8; col.owners = {vals[c]}; break;
-        case CSV_BOOL: col.field.type = DType::Bool; col.field.format = "b"; set_bool_values(col, vals[c], n, stream); break;
-        default: {
-          // a field's bytes lie inside its line, so the batch's byte span (at most 2 GiB, checked above) bounds the column
-          const Varlen v = varlen_layout((const int32_t*)slen[c].get(), n, nullptr, byte1 - byte0, "file input: column '" + names[c] + "'", stream);
-          if (n) {
-            KernelTimer t("csv_strings_kernel", stream);
-            csv_strings_kernel<<<grid_of(n), 256, 0, stream>>>(P.data, n, (const int32_t*)v.offsets.get(), (const long long*)ssrc[c].get(), (const int32_t*)sraw[c].get(), (uint8_t*)v.bytes.get());
-          }
-          col.field.type = DType::Utf8; col.field.format = "u";
-          set_varlen(col, v);
-          break;
-        }
-      }
-      set_validity_exact(col, (const uint8_t*)valid[c].get(), n, stream);
-      b.cols.push_back(std::move(col));
-    }
+    for (int c = 0; c < nc; ++c)
+      b.cols.push_back(finish_column(cols[c], Field{names[c], dtype[types[c]], true, dtype_arrow_format(dtype[types[c]])}, [&](const StagedColumn& s, uint8_t* bytes) {
+        if (!n) return;
+        KernelTimer t("csv_strings_kernel", stream);
+        csv_strings_kernel<<<grid_of(n), 256, 0, stream>>>(P.data, n, (const int32_t*)s.offsets.get(), (const long long*)s.src.get(), (const int32_t*)s.raw.get(), bytes);
+      }, stream));
     return b;
   }
 };

@@ -20,7 +20,9 @@
 
 #include "bitmap.cuh"
 #include "bitmap.h"
+#include "decoded.h"
 #include "engine.h"
+#include "stage_store.cuh"
 #include "tma.cuh"
 #include "json_mini.h"
 #include "decimal.cuh"
@@ -765,64 +767,32 @@ const char* json_err_text(int code) {
   }
 }
 
-// A scalar column (values / strings / validity) of `rows` rows being decoded.
-struct FieldBufs { BufferPtr values, valid_bytes, str_len, str_src, str_raw, str_offsets; };
-
-void alloc_field(DType type, int64_t rows, FieldBufs& fb, JsonField& F, cudaStream_t stream) {
-  fb.valid_bytes = device_alloc((size_t)std::max<int64_t>(rows, 1));
-  F.valid_bytes = (uint8_t*)fb.valid_bytes.get();
-  if (type == DType::Int64 || type == DType::Float64) { fb.values = device_alloc((size_t)std::max<int64_t>(rows, 1) * 8); F.values = fb.values.get(); }
-  else if (type == DType::Bool) { fb.values = device_alloc((size_t)std::max<int64_t>(rows, 1)); F.values = fb.values.get(); }
-  else if (type == DType::Utf8 || type == DType::List || type == DType::Struct) {
-    fb.str_len = device_alloc((size_t)(rows + 1) * 4); fb.str_src = device_alloc((size_t)std::max<int64_t>(rows, 1) * 8);
-    fb.str_raw = device_alloc((size_t)std::max<int64_t>(rows, 1) * 4);
-    ARK_CUDA(cudaMemsetAsync((int32_t*)fb.str_len.get() + rows, 0, 4, stream));  // the scan reads rows + 1 entries
-    F.str_len = (int32_t*)fb.str_len.get(); F.str_src = (long long*)fb.str_src.get(); F.str_raw_len = (int32_t*)fb.str_raw.get();
-  }
-}
-
-// Finishes a scalar column whose decode pass has run: validity bitmap, Boolean bit packing, string bytes.
-// `data` is the byte base str_src refers to, `data_bytes` the bytes of the input Binary column there.  Synchronises the
-// stream (string totals / null counts).
-Column finish_scalar(const std::string& name, DType type, int64_t rows, FieldBufs& fb, const uint8_t* data, int64_t data_bytes, cudaStream_t stream) {
-  Column c;
-  c.field.name = name; c.field.type = type; c.field.nullable = true; c.length = rows;
-  if (type == DType::Null) { c.field.format = "n"; return c; }
-  BufferPtr nulls = device_alloc(16), h = pinned_alloc(32);
-  ARK_CUDA(cudaMemsetAsync(nulls.get(), 0, 16, stream));
-  BufferPtr vbits = pack_bits((const uint8_t*)fb.valid_bytes.get(), rows, (unsigned long long*)nulls.get(), stream);
-  ARK_CUDA(cudaMemcpyAsync(h.get(), nulls.get(), 8, cudaMemcpyDeviceToHost, stream));
-  if (type == DType::Utf8) {
-    // a decoded string is never longer than its raw span inside the input column
-    varlen_guard((const int32_t*)fb.str_len.get(), rows, data_bytes, "json_to_arrow: column '" + name + "'", stream);
-    fb.str_offsets = varlen_scan((const int32_t*)fb.str_len.get(), rows, stream);
-    ARK_CUDA(cudaMemcpyAsync((char*)h.get() + 8, (int32_t*)fb.str_offsets.get() + rows, 4, cudaMemcpyDeviceToHost, stream));
-  }
-  ARK_CUDA(cudaStreamSynchronize(stream));
-  if (type == DType::Int64 || type == DType::Float64) {
-    c.data = (const uint8_t*)fb.values.get(); c.data_bytes = rows * 8; c.owners = {fb.values};
-  } else if (type == DType::Bool) {
-    set_bool_values(c, fb.values, rows, stream);
-  } else if (type == DType::Utf8) {
-    const int32_t total = *(const int32_t*)((char*)h.get() + 8);
-    BufferPtr bytes = device_alloc((size_t)total + 16);
-    if (rows) {
-      KernelTimer t("json_strings_kernel", stream);
-      json_strings_kernel<<<(unsigned)ceil_div(rows, 256), 256, 0, stream>>>(data, (const long long*)fb.str_src.get(), (const int32_t*)fb.str_raw.get(),
-                                                                            (const int32_t*)fb.str_offsets.get(), rows, (uint8_t*)bytes.get());
-    }
-    set_varlen(c, {fb.str_offsets, bytes, total});
-  }
-  set_validity(c, vbits, *(const long long*)h.get());
-  return c;
-}
-
 [[noreturn]] void raise_json(int code, int where, const char* what) {
   fail(ARK_ERR_PROCESS, std::string(json_err_text(code)) + " (" + what + " " + std::to_string(where) + ")");
 }
 
-// List<primitive> column from the raw spans of its rows (fb.str_src / fb.str_raw hold them, fb.valid_bytes the row validity)
-Column finish_list(const InferredField& f, int64_t rows, FieldBufs& fb, const uint8_t* data, int64_t data_bytes, cudaStream_t stream) {
+// A column of `rows` rows for the parse or List fill kernel.  `data_bytes`, the bytes of the input Binary column, bounds a
+// Utf8 column: a decoded string is never longer than its raw span there.
+StagedColumn stage_json(const std::string& name, DType type, int64_t rows, int64_t data_bytes, cudaStream_t stream) {
+  StagedColumn s = stage_column(type, rows, true, true, stream);
+  s.bound = data_bytes;
+  s.what = "json_to_arrow: column '" + name + "'";
+  return s;
+}
+
+// The Column of a settled scalar or Null column; `data` is the byte base its str_src refers to.
+Column json_column(const std::string& name, const StagedColumn& s, const uint8_t* data, cudaStream_t stream) {
+  return finish_column(s, Field{name, s.type, true, s.type == DType::Null ? "n" : ""}, [&](const StagedColumn& s, uint8_t* bytes) {
+    if (!s.rows) return;
+    KernelTimer t("json_strings_kernel", stream);
+    json_strings_kernel<<<(unsigned)ceil_div(s.rows, 256), 256, 0, stream>>>(data, (const long long*)s.src.get(), (const int32_t*)s.raw.get(),
+                                                                             (const int32_t*)s.offsets.get(), s.rows, bytes);
+  }, stream);
+}
+
+// List<primitive> column from the raw spans of the rows of the settled `s` (s.src / s.raw)
+Column finish_list(const InferredField& f, const StagedColumn& s, const uint8_t* data, int64_t data_bytes, cudaStream_t stream) {
+  const int64_t rows = s.rows;
   BufferPtr err = device_alloc(16), h = pinned_alloc(32);
   ARK_CUDA(cudaMemsetAsync(err.get(), 0, 16, stream));
   BufferPtr counts = device_alloc((size_t)(rows + 1) * 4);
@@ -830,7 +800,7 @@ Column finish_list(const InferredField& f, int64_t rows, FieldBufs& fb, const ui
   const unsigned g = (unsigned)std::max<int64_t>(1, ceil_div(rows, 128));
   if (rows) {
     KernelTimer t("json_list_count_kernel", stream);
-    json_list_count_kernel<<<g, 128, 0, stream>>>(data, (const long long*)fb.str_src.get(), (const int32_t*)fb.str_raw.get(), rows, (int32_t*)counts.get(), (int32_t*)err.get());
+    json_list_count_kernel<<<g, 128, 0, stream>>>(data, (const long long*)s.src.get(), (const int32_t*)s.raw.get(), rows, (int32_t*)counts.get(), (int32_t*)err.get());
   }
   // every element takes at least one byte of its row's raw span inside the input column
   varlen_guard((const int32_t*)counts.get(), rows, data_bytes, "json_to_arrow: column '" + f.name + "'", stream);
@@ -840,25 +810,24 @@ Column finish_list(const InferredField& f, int64_t rows, FieldBufs& fb, const ui
   ARK_CUDA(cudaStreamSynchronize(stream));
   if (((int32_t*)((char*)h.get() + 8))[0]) raise_json(((int32_t*)((char*)h.get() + 8))[0], ((int32_t*)((char*)h.get() + 8))[1], "row");
   const int64_t total = *(const int32_t*)h.get();
-  FieldBufs cb;
-  JsonField CF;
-  memset(&CF, 0, sizeof CF);
-  alloc_field(f.elem, total, cb, CF, stream);
+  std::vector<StagedColumn> item = {stage_json("item", f.elem, total, data_bytes, stream)};  // arrow-rs names a list's field "item"
+  const StagedColumn& e = item[0];
   if (rows && total) {
     KernelTimer t("json_list_fill_kernel", stream);
-    json_list_fill_kernel<<<g, 128, 0, stream>>>(data, (const long long*)fb.str_src.get(), (const int32_t*)fb.str_raw.get(), rows, (const int32_t*)offs.get(), (int)f.elem,
-                                                 CF.values, CF.valid_bytes, CF.str_len, CF.str_src, CF.str_raw_len, (int32_t*)err.get());
+    json_list_fill_kernel<<<g, 128, 0, stream>>>(data, (const long long*)s.src.get(), (const int32_t*)s.raw.get(), rows, (const int32_t*)offs.get(), (int)f.elem,
+                                                 e.values.get(), (uint8_t*)e.valid.get(), (int32_t*)e.len.get(), (long long*)e.src.get(), (int32_t*)e.raw.get(),
+                                                 (int32_t*)err.get());
   }
-  ARK_CUDA(cudaMemcpyAsync((char*)h.get() + 8, err.get(), 8, cudaMemcpyDeviceToHost, stream));
-  ARK_CUDA(cudaStreamSynchronize(stream));
-  if (((int32_t*)((char*)h.get() + 8))[0]) raise_json(((int32_t*)((char*)h.get() + 8))[0], ((int32_t*)((char*)h.get() + 8))[1], "row");
-  Column child = finish_scalar("item", f.elem, total, cb, data, data_bytes, stream);  // arrow-rs names a list's field "item"
+  settle_columns(item, err.get(), 8, [](const void* h) {
+    const int32_t* e = (const int32_t*)h;
+    if (e[0]) raise_json(e[0], e[1], "row");
+  }, stream);
   Column c;
   c.field.name = f.name; c.field.type = DType::List; c.field.format = "+l"; c.field.nullable = true; c.length = rows;
-  set_validity_exact(c, (const uint8_t*)fb.valid_bytes.get(), rows, stream);
+  set_validity(c, s.bits, s.null_count);
   c.offsets = (const int32_t*)offs.get(); c.first_offset = 0;
   c.owners.push_back(offs);
-  c.children.push_back(std::move(child));
+  c.children.push_back(json_column("item", e, data, stream));
   return c;
 }
 
@@ -920,19 +889,13 @@ const std::string& json_to_arrow_value_field(const Processor& p) { return static
 
 namespace {
 
-// Uploads the field table of `specs` (names included) and returns the parameter block's view of it.
-struct FieldTable {
-  std::vector<FieldBufs> fb;
-  BufferPtr table_dev, names_dev;  // only for schemas that do not fit the parameter block
-};
-
 // Decodes `specs` into `rows` rows.  The payloads are rows of a Binary column (P.offsets) or raw spans (P.span_src).
 // optimistic: payload i → row i in ONE pass; returns false (nothing raised) when the batch is not of that shape or
 // holds an error — the caller then takes the two-pass route, which reports errors the canonical way.
 bool decode_fields(const std::vector<InferredField>& specs, JsonParams Q, unsigned grid, size_t smem, int64_t rows, bool optimistic,
                    const long long* row_start, const uint8_t* data, int64_t data_bytes, std::vector<Column>& out_cols, cudaStream_t stream) {
   const size_t nf = specs.size();
-  std::vector<FieldBufs> fb(nf);
+  std::vector<StagedColumn> cols;
   std::vector<JsonField> table(nf);
   // names longer than the inline slot live in one HBM pool
   std::string pool;
@@ -949,7 +912,10 @@ bool decode_fields(const std::vector<InferredField>& specs, JsonParams Q, unsign
     F.dtype = (int)specs[k].type; F.name_len = (int)specs[k].name.size();
     if ((int)specs[k].name.size() > JS_MAX_NAME) F.long_name = (const char*)names_dev.get() + pool_off[k];
     else memcpy(F.name, specs[k].name.data(), specs[k].name.size());
-    alloc_field(specs[k].type, rows, fb[k], F, stream);
+    cols.push_back(stage_json(specs[k].name, specs[k].type, rows, data_bytes, stream));
+    const StagedColumn& s = cols.back();
+    F.values = s.values.get(); F.valid_bytes = (uint8_t*)s.valid.get();
+    F.str_len = (int32_t*)s.len.get(); F.str_src = (long long*)s.src.get(); F.str_raw_len = (int32_t*)s.raw.get();
   }
   Q.n_fields = (int)nf;
   Q.row_start = row_start;
@@ -990,16 +956,18 @@ bool decode_fields(const std::vector<InferredField>& specs, JsonParams Q, unsign
     ARK_CUDA(cudaStreamSynchronize(stream));
     if (e[0] != JE_NONE) raise_json(e[0], e[1], "row");
   }
+  // every scalar column of the level and the validity of its List / Struct columns come back in one round trip
+  settle_columns(cols, nullptr, 0, nullptr, stream);
   out_cols.clear();
   for (size_t k = 0; k < nf; ++k) {
     const InferredField& f = specs[k];
-    if (f.type == DType::List) out_cols.push_back(finish_list(f, rows, fb[k], data, data_bytes, stream));
+    if (f.type == DType::List) out_cols.push_back(finish_list(f, cols[k], data, data_bytes, stream));
     else if (f.type == DType::Struct) {
       // the struct's children: the same decoder over the captured spans, one row per span
       JsonParams S;
       memset(&S, 0, sizeof S);
       S.data = data; S.n_payloads = rows; S.stage_bytes = 0;
-      S.span_src = (const long long*)fb[k].str_src.get(); S.span_len = (const int32_t*)fb[k].str_raw.get();
+      S.span_src = (const long long*)cols[k].src.get(); S.span_len = (const int32_t*)cols[k].raw.get();
       std::vector<Column> kids;
       if (rows > 0 && !f.kids.empty()) {
         if (!decode_fields(f.kids, S, (unsigned)ceil_div(rows, JS_THREADS), 32, rows, true, nullptr, data, data_bytes, kids, stream))
@@ -1009,10 +977,10 @@ bool decode_fields(const std::vector<InferredField>& specs, JsonParams Q, unsign
       }
       Column c;
       c.field.name = f.name; c.field.type = DType::Struct; c.field.format = "+s"; c.field.nullable = true; c.length = rows;
-      set_validity_exact(c, (const uint8_t*)fb[k].valid_bytes.get(), rows, stream);
+      set_validity(c, cols[k].bits, cols[k].null_count);
       c.children = std::move(kids);
       out_cols.push_back(std::move(c));
-    } else out_cols.push_back(finish_scalar(f.name, f.type, rows, fb[k], data, data_bytes, stream));
+    } else out_cols.push_back(json_column(f.name, cols[k], data, stream));
   }
   ARK_CUDA(cudaGetLastError());
   ARK_CUDA(cudaStreamSynchronize(stream));
@@ -1080,10 +1048,8 @@ Batch json_to_arrow_device(const Processor& proc, Batch& in, cudaStream_t stream
   memset(&P, 0, sizeof P);
   P.data = col.data; P.offsets = col.offsets; P.validity = col.validity; P.validity_bit0 = col.validity_bit0;
   P.n_payloads = n;
-  // staging window: the CTA's payload bytes + alignment slack; payloads that average more than 256 bytes are parsed in place
   static const bool no_stage = getenv("ARK_JSON_NO_STAGE") != nullptr;
-  const double avg = (double)col.data_bytes / (double)n;
-  P.stage_bytes = (!no_stage && avg <= 256.0) ? (int)round_up((int64_t)(avg * JS_THREADS * 1.25) + 256, 1024) : 0;
+  P.stage_bytes = no_stage ? 0 : record_stage_window(col.data_bytes, n, JS_THREADS);
   const size_t smem = (size_t)P.stage_bytes + 32;
   const unsigned grid = (unsigned)ceil_div(n, JS_THREADS);
 

@@ -36,7 +36,7 @@
 #include <algorithm>
 
 #include "bitmap.cuh"
-#include "bitmap.h"
+#include "decoded.h"
 #include "engine.h"
 #include "json_mini.h"
 #include "proto_schema.h"
@@ -459,7 +459,6 @@ Batch protobuf_to_arrow_device(const Processor& proc, Batch& in, cudaStream_t st
   std::vector<int> vl = {ci};
   resolve_varlen_extents(in, vl, stream);
   const int64_t n = col.length;
-  BufferPtr h = pinned_alloc(16 + 4 * PB_MAX_FIELDS);
 
   // ---- output rows: the non-NULL payloads ----
   int64_t rows = n;
@@ -472,6 +471,7 @@ Batch protobuf_to_arrow_device(const Processor& proc, Batch& in, cudaStream_t st
       protobuf_valid_kernel<<<(unsigned)ceil_div(n, 256), 256, 0, stream>>>(col.validity, col.validity_bit0, n, (int32_t*)flags.get());
     }
     row_of = varlen_scan((const int32_t*)flags.get(), n, stream);
+    BufferPtr h = pinned_alloc(8);
     ARK_CUDA(cudaMemcpyAsync(h.get(), (int32_t*)row_of.get() + n, 4, cudaMemcpyDeviceToHost, stream));
     ARK_CUDA(cudaStreamSynchronize(stream));
     rows = *(const int32_t*)h.get();
@@ -487,7 +487,7 @@ Batch protobuf_to_arrow_device(const Processor& proc, Batch& in, cudaStream_t st
   P.row_of = (const int32_t*)row_of.get();
   memset(P.by_number, -1, sizeof P.by_number);
   const size_t nf = fields.size();
-  std::vector<BufferPtr> values(nf), src(nf), lens(nf);
+  std::vector<StagedColumn> cols;
   for (size_t k = 0; k < nf; ++k) {
     const PbField& f = fields[k];
     PbDecField& F = P.fields[k];
@@ -495,19 +495,14 @@ Batch protobuf_to_arrow_device(const Processor& proc, Batch& in, cudaStream_t st
     if (f.oneof >= 0)
       for (size_t j = 0; j < nf; ++j) if (j != k && fields[j].oneof == f.oneof) F.others |= 1ull << j;
     if (f.number < PB_BY_NUMBER) P.by_number[f.number] = (int8_t)k;
-    const DType t = arrow_type_of(f.kind);
-    if (t == DType::Utf8 || t == DType::Binary) {
-      src[k] = device_alloc((size_t)std::max<int64_t>(rows, 1) * 8);
-      lens[k] = device_alloc((size_t)(rows + 1) * 4);
-      ARK_CUDA(cudaMemsetAsync((int32_t*)lens[k].get() + rows, 0, 4, stream));  // the scan reads rows + 1 entries
-      F.str_src = (long long*)src[k].get(); F.str_len = (int32_t*)lens[k].get();
-      F.dflt = ((uint64_t)pp.default_off[k] << 32) | (uint64_t)f.default_bytes.size();
-    } else {
-      F.width = t == DType::Bool ? 1 : (uint8_t)fixed_width(t);
-      values[k] = device_alloc((size_t)std::max<int64_t>(rows, 1) * F.width);
-      F.values = values[k].get();
-      F.dflt = f.default_bits;
-    }
+    cols.push_back(stage_column(arrow_type_of(f.kind), rows, false, false, stream));
+    StagedColumn& s = cols.back();
+    F.values = s.values.get(); F.str_src = (long long*)s.src.get(); F.str_len = (int32_t*)s.len.get();
+    F.width = !s.values ? 0 : s.type == DType::Bool ? 1 : (uint8_t)fixed_width(s.type);
+    F.dflt = s.len ? ((uint64_t)pp.default_off[k] << 32) | (uint64_t)f.default_bytes.size() : f.default_bits;
+    // a row's span lies inside its own payload, so the payload bytes plus one default per row bound a string column
+    s.bound = col.data_bytes + rows * (int64_t)f.default_bytes.size();
+    s.what = "protobuf_to_arrow: column '" + f.name + "'";
   }
   BufferPtr err = device_alloc(8), blob;
   ARK_CUDA(cudaMemsetAsync(err.get(), 0xFF, 8, stream));
@@ -517,50 +512,25 @@ Batch protobuf_to_arrow_device(const Processor& proc, Batch& in, cudaStream_t st
     ARK_CUDA(cudaMemcpyAsync(blob.get(), pp.default_blob.data(), pp.default_blob.size(), cudaMemcpyHostToDevice, stream));
   }
   if (rows > 0) {
-    // staging window: the CTA's payload bytes + alignment slack; payloads that average more than 256 bytes are parsed in place
-    const double avg = (double)col.data_bytes / (double)n;
-    P.stage_bytes = avg <= 256.0 ? (int)round_up((int64_t)(avg * PB_THREADS * 1.25) + 256, 1024) : 0;
+    P.stage_bytes = record_stage_window(col.data_bytes, n, PB_THREADS);
     KernelTimer t("protobuf_decode_kernel", stream);
     protobuf_decode_kernel<<<(unsigned)ceil_div(n, PB_THREADS), PB_THREADS, (size_t)P.stage_bytes + 32, stream>>>(P);
   }
   ARK_CUDA(cudaGetLastError());
-  // the error word and every string column's byte total come back in one round trip
-  std::vector<BufferPtr> str_offs(nf);
-  ARK_CUDA(cudaMemcpyAsync(h.get(), err.get(), 8, cudaMemcpyDeviceToHost, stream));
-  for (size_t k = 0; k < nf; ++k) {
-    if (!lens[k]) continue;
-    str_offs[k] = varlen_scan((const int32_t*)lens[k].get(), rows, stream);
-    ARK_CUDA(cudaMemcpyAsync((char*)h.get() + 16 + 4 * k, (int32_t*)str_offs[k].get() + rows, 4, cudaMemcpyDeviceToHost, stream));
-  }
-  ARK_CUDA(cudaStreamSynchronize(stream));
-  const unsigned long long e = *(const unsigned long long*)h.get();
-  if (e != ~0ull)
-    fail(ARK_ERR_PROCESS, std::string("Protobuf message parsing failed: ") + pb_err_text((int)(e & 0xFF)) + " (payload " + std::to_string(e >> 8) + ")");
-  // a row's span lies inside its own payload, so the payload bytes plus one default per row bound a string column's total
-  for (size_t k = 0; k < nf; ++k)
-    if (lens[k])
-      varlen_guard((const int32_t*)lens[k].get(), rows, col.data_bytes + rows * (int64_t)fields[k].default_bytes.size(),
-                     "protobuf_to_arrow: column '" + fields[k].name + "'", stream);
+  settle_columns(cols, err.get(), 8, [](const void* h) {
+    const unsigned long long e = *(const unsigned long long*)h;
+    if (e != ~0ull)
+      fail(ARK_ERR_PROCESS, std::string("Protobuf message parsing failed: ") + pb_err_text((int)(e & 0xFF)) + " (payload " + std::to_string(e >> 8) + ")");
+  }, stream);
 
   // ---- columns ----
   Batch out;
   out.num_rows = rows;
   for (size_t k = 0; k < nf; ++k) {
     const DType t = arrow_type_of(fields[k].kind);
-    Column c;
-    c.field.name = fields[k].name; c.field.type = t; c.field.nullable = false; c.field.format = dtype_arrow_format(t);
-    c.length = rows;
-    if (str_offs[k]) {
-      const int32_t total = *(const int32_t*)((char*)h.get() + 16 + 4 * k);
-      BufferPtr bytes = device_alloc((size_t)total + 16);
-      if (total) launch_span_copy(col.data, (const uint8_t*)blob.get(), (const long long*)src[k].get(), (const int32_t*)str_offs[k].get(), rows, (uint8_t*)bytes.get(), stream);
-      set_varlen(c, {str_offs[k], bytes, total});
-    } else if (t == DType::Bool) {
-      set_bool_values(c, values[k], rows, stream);
-    } else {
-      c.data = (const uint8_t*)values[k].get(); c.data_bytes = rows * fixed_width(t); c.owners = {values[k]};
-    }
-    out.cols.push_back(std::move(c));
+    out.cols.push_back(finish_column(cols[k], Field{fields[k].name, t, false, dtype_arrow_format(t)}, [&](const StagedColumn& s, uint8_t* bytes) {
+      if (s.total) launch_span_copy(col.data, (const uint8_t*)blob.get(), (const long long*)s.src.get(), (const int32_t*)s.offsets.get(), rows, bytes, stream);
+    }, stream));
   }
   ARK_CUDA(cudaGetLastError());
   ARK_CUDA(cudaStreamSynchronize(stream));

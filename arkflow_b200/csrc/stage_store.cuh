@@ -30,4 +30,12 @@ inline int stage_window(int64_t total, int64_t n, int rows_per_cta) {
   return (int)std::min<int64_t>(44 * 1024, round_up((int64_t)((double)total / (double)n * rows_per_cta * 1.5) + 256, 1024));
 }
 
+// Staging window of a decode kernel whose CTAs of `threads` threads parse one record each from `bytes` bytes of `n`
+// records: the average CTA's bytes + 25 % + alignment slack, or 0 when records average more than 256 bytes (every CTA
+// parses in place).
+inline int record_stage_window(int64_t bytes, int64_t n, int threads) {
+  const double avg = (double)bytes / (double)n;
+  return avg <= 256.0 ? (int)round_up((int64_t)(avg * threads * 1.25) + 256, 1024) : 0;
+}
+
 }  // namespace ark

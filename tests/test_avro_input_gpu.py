@@ -247,6 +247,8 @@ def blocks_with(bad_block, bad, codec="null", n_blocks=5, per=6):
 def test_bad_record(timing, tmp_path, kind, where):
     want, err = check(timing, tmp_path, blocks_with(where, BAD_RECORDS[kind]), batch_size=4)
     assert err is not None and err.kind == "Process" and (" in record %d " % (where * 6 + 2)) in err.message
+    # each good read before it copies its `s` and `y` bytes; the failing read copies nothing
+    assert launches(timing, "protobuf_strings_kernel") == 2 * ((where * 6 + 2) // 4)
 
 
 @pytest.mark.parametrize("where", [0, 2, 4])

@@ -345,8 +345,10 @@ def lines(*parts):
     (b"x,1.5,true,\xff,extra", "Csv error: incorrect number of fields for line 1202"),
     (b"5,1.5,maybe,\xff", "Parser error: Error while parsing value of line 1202"),
 ])
-def test_csv_errors_carry_the_message_and_the_physical_line(tmp_path, bad, message):
+def test_csv_errors_carry_the_message_and_the_physical_line(timing, tmp_path, bad, message):
+    timing.ark_kernel_timing_reset()
     expect_error(tmp_path, lines(good(1200), [bad], good(300, 1200)), message)
+    assert launches(timing, "csv_strings_kernel") == 0  # the failing batch (the file's only one) copies no string
 
 
 def test_csv_invalid_utf8_in_the_header_and_in_the_sample(tmp_path):

@@ -17,6 +17,7 @@ from oracle import protobuf_oracle as O
 from oracle.json_oracle import json_to_arrow
 from oracle.protobuf_oracle import PbField
 from oracle.sql_oracle import sql_process
+from test_inputs_edges_gpu import launches
 
 pytestmark = pytest.mark.gpu
 
@@ -471,6 +472,16 @@ def test_string_column_beyond_int32_offsets_is_an_error(gpu, tmp_path, rows):
     with pytest.raises(ArkError) as e:
         decode(dec, [b""] * rows)
     assert e.value.kind == "Process" and "2 GiB" in e.value.message, e.value.message
+    # a malformed payload in the same batch is reported first, before the lengths are summed
+    gpu.ark_kernel_timing_enable(1)
+    gpu.ark_kernel_timing_reset()
+    try:
+        with pytest.raises(ArkError) as e:
+            decode(dec, [b""] * (rows - 1) + [b"\x0a"])
+        assert launches(gpu, "protobuf_sum64_kernel") == 0 and launches(gpu, "protobuf_strings_kernel") == 0
+    finally:
+        gpu.ark_kernel_timing_enable(0)
+    assert e.value.kind == "Process" and e.value.message.startswith("Protobuf message parsing failed: "), e.value.message
 
 
 def _pattern_bytes(n):
