@@ -169,6 +169,7 @@ int ark_sql_partial_aggregate_device(ark_proc_t* p, ArrowDeviceArray* in, ArrowS
     if (bound->plan->kind != Plan::Aggregate) fail(ARK_ERR_PROCESS, "partial aggregate requested for a query without aggregation");
     StreamLease lease;
     Batch b = import_device(&view, in_schema, &bound->mask, in_owner, false, &bound->fields);
+    if (!bound->plan->derived.empty()) b = append_json_columns(*bound->plan, b, lease.s);
     std::vector<int64_t> rows;
     ExportAllocScope exported;  // the partial states are published to the other ranks over CUDA IPC
     Batch r = run_partial_aggregate(*bound->plan, b, n_parts, rows, lease.s);

@@ -19,6 +19,7 @@ std::unique_ptr<SqlProcessor> SqlProcessor::from_config(const char* config_json)
   if (q->kind != JsonValue::String) fail(ARK_ERR_SERIALIZATION, "invalid type for `query`: expected a string");
   auto p = std::make_unique<SqlProcessor>();
   p->query_text = q->str;
+  p->json_functions = true;  // sql.rs:18-24 registers datafusion-functions-json
   if (const JsonValue* t = cfg.get("table_name")) {
     if (t->kind == JsonValue::String) p->table_name = t->str;
     else if (t->kind != JsonValue::Null) fail(ARK_ERR_SERIALIZATION, "invalid type for `table_name`: expected a string");
@@ -44,7 +45,7 @@ std::shared_ptr<const Plan> SqlProcessor::plan_for(const std::vector<Field>& fie
     auto it = plans_.find(key);
     if (it != plans_.end()) { if (it->second->kind == Plan::Aggregate) last_agg_ = it->second; return it->second; }
   }
-  auto plan = std::make_shared<Plan>(bind_query(ast, table_name, fields));
+  auto plan = std::make_shared<Plan>(bind_query(ast, table_name, fields, json_functions));
   std::lock_guard<std::mutex> l(mu_);
   if (plans_.size() > 64) plans_.clear();
   plans_[key] = plan;
@@ -55,7 +56,8 @@ std::shared_ptr<const Plan> SqlProcessor::plan_for(const std::vector<Field>& fie
 std::vector<bool> needed_mask(const Plan& plan, size_t n_fields) {
   std::vector<bool> m(n_fields, false);
   if (plan.identity) { std::fill(m.begin(), m.end(), true); return m; }
-  for (int c : plan.used_cols) m[c] = true;
+  for (int c : plan.used_cols) if ((size_t)c < n_fields) m[c] = true;  // the others are derived columns
+  for (auto& d : plan.derived) m[d.doc_col] = true;
   return m;
 }
 
@@ -108,7 +110,10 @@ std::shared_ptr<const Plan> SqlProcessor::join_plan_for(const std::vector<std::s
   return plan;
 }
 
-Batch SqlProcessor::execute(const Plan& plan, Batch& in, cudaStream_t stream) {
+Batch SqlProcessor::execute(const Plan& plan, Batch& batch, cudaStream_t stream) {
+  Batch with_json;
+  if (!plan.derived.empty()) with_json = append_json_columns(plan, batch, stream);
+  Batch& in = plan.derived.empty() ? batch : with_json;
   switch (plan.kind) {
     case Plan::FilterProject: {
       Batch r = run_filter_project(plan, in, stream);

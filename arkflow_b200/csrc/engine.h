@@ -42,6 +42,7 @@ struct SqlProcessor : Processor {
   std::string query_text;
   std::string table_name = "flow";  // DEFAULT_TABLE_NAME, sql.rs:38
   Query ast;
+  bool json_functions = false;      // the json_* calls bind (processors built from a config; not expression evaluation)
 
   // config_json as documented at ark_sql_create
   static std::unique_ptr<SqlProcessor> from_config(const char* config_json);
@@ -59,7 +60,8 @@ struct SqlProcessor : Processor {
   struct BoundSchema { std::vector<Field> fields; std::shared_ptr<const Plan> plan; std::vector<bool> mask; };
   std::shared_ptr<const BoundSchema> bind(const ArrowSchema* schema);
 
-  // Runs the bound plan on an HBM-resident batch.  `in` must contain the plan's used columns.
+  // Runs the bound plan on an HBM-resident batch.  `in` must contain the plan's used columns and the documents of its
+  // derived columns.
   Batch execute(const Plan& plan, Batch& in, cudaStream_t stream);
 
  private:
@@ -72,7 +74,14 @@ struct SqlProcessor : Processor {
 // Which of `n_fields` input columns the plan reads (all of them for SELECT *).
 std::vector<bool> needed_mask(const Plan& plan, size_t n_fields);
 
+// `in` with the plan's derived columns appended, filled from their documents by one json_path_kernel launch per
+// document column and up to JSON_MAX_CALLS calls (json_path.cu).
+Batch append_json_columns(const Plan& plan, const Batch& in, cudaStream_t stream);
 Batch run_filter_project(const Plan& plan, Batch& in, cudaStream_t stream);
+struct StagedColumn;  // decoded.h
+// The bytes of a settled Utf8 column whose row r is the JSON text data[src[r] ..] of raw[r] bytes, a negative raw
+// meaning |raw| bytes of a string body whose escapes are decoded (json.cu).
+void launch_json_strings(const uint8_t* data, const StagedColumn& s, uint8_t* bytes, cudaStream_t stream);
 Batch run_aggregate(const Plan& plan, Batch& in, cudaStream_t stream);
 Batch run_join(const Plan& plan, Batch& left, Batch& right, cudaStream_t stream);
 Batch run_partial_aggregate(const Plan& plan, Batch& in, int n_parts, std::vector<int64_t>& part_rows, cudaStream_t stream);

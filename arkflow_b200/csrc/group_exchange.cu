@@ -363,6 +363,7 @@ int ark_sql_group_by_push_device(ark_proc_t* p, ark_dist_t* d, ArrowDeviceArray*
     if (bound->plan->kind != Plan::Aggregate) fail(ARK_ERR_PROCESS, "not an aggregate query");
     StreamLease lease;
     Batch b = import_device(&view, in_schema, &bound->mask, in_owner, false, &bound->fields);
+    if (!bound->plan->derived.empty()) b = append_json_columns(*bound->plan, b, lease.s);
     ++c.step;
     c.pushed = true;
     run_group_by_push(*bound->plan, b, c, lease.s);

@@ -95,9 +95,31 @@ struct AggHints {
   std::vector<CachedTable> cache;
 };
 
+// The JSON path functions of datafusion-functions-json 0.47 (DESIGN.md §6).
+enum class JsonFn : uint8_t { GetStr, GetInt, GetFloat, GetBool, GetJson, AsText, Contains, Length };
+
+struct JsonPathElem {
+  bool is_key = true;
+  std::string key;     // an object key, matched against each key with its escapes decoded
+  int64_t index = 0;   // an array index (>= 0)
+};
+
+// One distinct json_* call of the query.  The planner replaces it by a column appended after the input fields
+// (input_fields[n_input_fields + i] for derived[i]); json_path.cu fills every derived column before the plan runs, so
+// the row kernels and the aggregate only ever see ordinary columns.
+struct DerivedCol {
+  JsonFn fn = JsonFn::GetStr;
+  int doc_col = -1;          // the input column holding the documents
+  bool doc_cast = false;     // a Binary column read through CAST(.. AS STRING): invalid UTF-8 fails the query as the cast does
+  std::vector<JsonPathElem> path;  // at most JSON_MAX_PATH elements
+};
+constexpr int JSON_MAX_PATH = 8;
+
 struct Plan {
   enum Kind { FilterProject, Aggregate, Join } kind = FilterProject;
-  std::vector<Field> input_fields;   // of table 0
+  std::vector<Field> input_fields;   // of table 0, then one per derived column
+  size_t n_input_fields = 0;         // the batch's own columns
+  std::vector<DerivedCol> derived;
   std::vector<int> used_cols;        // slot → input column index (kernels see only these)
   bool has_pred = false;
   VmProgram pred{};
@@ -126,8 +148,9 @@ struct Plan {
 
 // Throws ARK_ERR_PROCESS ("Execution query error: …") for binding errors the reference would raise
 // at plan time (unknown column/table, type errors) and ARK_ERR_UNSUPPORTED for constructs outside
-// the GPU subset.
-Plan bind_query(const Query& q, const std::string& table_name, const std::vector<Field>& fields);
+// the GPU subset.  `json_functions`: the json_* calls bind (the sql processor and the file input's query register
+// datafusion-functions-json; a bare SessionContext, as expression evaluation uses, does not).
+Plan bind_query(const Query& q, const std::string& table_name, const std::vector<Field>& fields, bool json_functions = false);
 Plan bind_join(const Query& q, const std::vector<std::string>& names,
                const std::vector<std::vector<Field>>& tables);
 

@@ -47,15 +47,17 @@ std::string fmt_f64(double v) {
 
 struct Binder {
   std::string table;                 // visible table name (alias or name)
-  const std::vector<Field>* fields;
+  const std::vector<Field>* fields;  // the input's fields, then the derived columns' (Plan::input_fields)
+  size_t n_input = 0;                // fields the query can name
   std::vector<int>* used;            // slot → column index
 
   int resolve(const Expr& e) const {
+    if (e.derived >= 0) return (int)n_input + e.derived;
     if (!e.qualifier.empty() && e.qualifier != table)
       plan_error("Schema error: No field named " + e.qualifier + "." + e.name + ".");
-    for (size_t i = 0; i < fields->size(); ++i) if ((*fields)[i].name == e.name) return (int)i;
+    for (size_t i = 0; i < n_input; ++i) if ((*fields)[i].name == e.name) return (int)i;
     std::string valid;
-    for (auto& f : *fields) { if (!valid.empty()) valid += ", "; valid += table + "." + f.name; }
+    for (size_t i = 0; i < n_input; ++i) { if (!valid.empty()) valid += ", "; valid += table + "." + (*fields)[i].name; }
     plan_error("Schema error: No field named " + e.name + ". Valid fields are " + valid + ".");
   }
   int slot_of(int col) const {
@@ -291,7 +293,7 @@ struct Binder {
 
 std::string display(const Expr& e, const std::string& table) {
   switch (e.kind) {
-    case Expr::Column: return (e.qualifier.empty() ? table : e.qualifier) + "." + e.name;
+    case Expr::Column: return e.derived >= 0 ? e.name : (e.qualifier.empty() ? table : e.qualifier) + "." + e.name;
     case Expr::Literal:
       switch (e.lit_type) {
         case DType::Null: return "NULL";
@@ -353,19 +355,120 @@ void bind_where(const Query& q, const Binder& b, Plan& plan) {
   detect_simple_predicate(*q.where, b, plan);
 }
 
+// ---- json_* calls → derived columns ----
+
+bool json_fn_of(const std::string& n, JsonFn* fn) {
+  static const std::pair<const char*, JsonFn> names[] = {
+      {"json_get_str", JsonFn::GetStr}, {"json_get_int", JsonFn::GetInt}, {"json_get_float", JsonFn::GetFloat},
+      {"json_get_bool", JsonFn::GetBool}, {"json_get_json", JsonFn::GetJson}, {"json_as_text", JsonFn::AsText},
+      {"json_contains", JsonFn::Contains}, {"json_length", JsonFn::Length}};
+  for (auto& p : names) if (n == p.first) { *fn = p.second; return true; }
+  return false;
+}
+
+// json_length is UInt64 in datafusion-functions-json; it is Int64 here, the column type the plan reads (DESIGN.md §6).
+DType json_result_type(JsonFn fn) {
+  switch (fn) {
+    case JsonFn::GetInt: case JsonFn::Length: return DType::Int64;
+    case JsonFn::GetFloat: return DType::Float64;
+    case JsonFn::GetBool: case JsonFn::Contains: return DType::Bool;
+    default: return DType::Utf8;
+  }
+}
+
+// Replaces every json_* call under `e` by a Column naming its derived column, one per distinct display name.
+void rewrite_json(ExprPtr& e, const Binder& b, Plan& plan) {
+  JsonFn fn;
+  if (e->kind != Expr::Func || !json_fn_of(e->name, &fn)) {
+    for (auto& a : e->args) rewrite_json(a, b, plan);
+    return;
+  }
+  const std::string what = e->name + "()";
+  if (e->distinct || e->star_arg || e->args.empty()) unsupported(what + " without a JSON document argument");
+  if (e->args.size() > 1 + (size_t)JSON_MAX_PATH) unsupported(what + " with more than " + std::to_string(JSON_MAX_PATH) + " path elements");
+  DerivedCol d;
+  d.fn = fn;
+  const Expr& doc = *e->args[0];
+  const Expr* col = doc.kind == Expr::Column ? &doc
+                  : doc.kind == Expr::Cast && doc.cast_to == DType::Utf8 && doc.args[0]->kind == Expr::Column ? doc.args[0].get()
+                  : nullptr;
+  const DType t = col && col->derived < 0 ? b.type_of(*col) : DType::Null;
+  if (t != DType::Utf8 && !(t == DType::Binary && col != &doc))
+    unsupported(what + ": the JSON document must be a Utf8 column or CAST(<Binary column> AS STRING)");
+  d.doc_col = b.resolve(*col);
+  d.doc_cast = t == DType::Binary;
+  for (size_t i = 1; i < e->args.size(); ++i) {
+    const Expr& a = *e->args[i];
+    JsonPathElem pe;
+    if (a.kind == Expr::Literal && a.lit_type == DType::Utf8) pe.key = a.str;
+    else if (a.kind == Expr::Literal && a.lit_type == DType::Int64 && a.i64 >= 0) { pe.is_key = false; pe.index = a.i64; }
+    else unsupported(what + ": a path element must be a string or non-negative integer literal");
+    d.path.push_back(pe);
+  }
+  auto c = std::make_unique<Expr>();
+  c->kind = Expr::Column;
+  c->name = display(*e, b.table);
+  for (size_t k = 0; k < plan.derived.size(); ++k)
+    if (plan.input_fields[b.n_input + k].name == c->name) c->derived = (int)k;
+  if (c->derived < 0) {
+    c->derived = (int)plan.derived.size();
+    const DType rt = json_result_type(fn);
+    plan.derived.push_back(d);
+    plan.input_fields.push_back(Field{c->name, rt, true, dtype_arrow_format(rt)});
+  }
+  e = std::move(c);
+}
+
+// A copy of `q` whose json_* calls are derived columns of `plan` (the parsed query serves every schema).
+Query rewrite_json_calls(const Query& q, const Binder& b, Plan& plan) {
+  auto take = [&](const ExprPtr& e) {
+    ExprPtr c = e ? e->clone() : nullptr;
+    if (c) rewrite_json(c, b, plan);
+    return c;
+  };
+  Query r;
+  r.from = q.from;
+  r.limit = q.limit;
+  for (auto& it : q.select) {
+    SelectItem s;
+    s.expr = take(it.expr); s.alias = it.alias; s.is_star = it.is_star; s.star_qualifier = it.star_qualifier;
+    r.select.push_back(std::move(s));
+  }
+  r.where = take(q.where);
+  for (auto& g : q.group_by) r.group_by.push_back(take(g));
+  for (auto& o : q.order_by) r.order_by.push_back(take(o));
+  return r;
+}
+
+Plan bind_single(const Query& q, Plan plan);
+
 }  // namespace
 
 std::string expr_display_name(const Expr& e, const std::string& table) { return display(e, table); }
 
-Plan bind_query(const Query& q, const std::string& table_name, const std::vector<Field>& fields) {
+Plan bind_query(const Query& q, const std::string& table_name, const std::vector<Field>& fields, bool json_functions) {
   if (!q.joins.empty()) unsupported("JOIN in a single-table processor call");
   if (q.from.name != table_name)
     plan_error("Error during planning: table '" + q.from.name + "' not found");
   Plan plan;
   plan.input_fields = fields;
+  plan.n_input_fields = fields.size();
+  if (json_functions) {
+    Binder b;
+    b.table = q.from.visible(); b.fields = &plan.input_fields; b.n_input = fields.size(); b.used = &plan.used_cols;
+    Query r = rewrite_json_calls(q, b, plan);
+    if (!plan.derived.empty()) return bind_single(r, std::move(plan));
+  }
+  return bind_single(q, std::move(plan));
+}
+
+namespace {
+
+Plan bind_single(const Query& q, Plan plan) {
+  const std::vector<Field>& fields = plan.input_fields;
   plan.limit = q.limit;
   Binder b;
-  b.table = q.from.visible(); b.fields = &fields; b.used = &plan.used_cols;
+  b.table = q.from.visible(); b.fields = &fields; b.n_input = plan.n_input_fields; b.used = &plan.used_cols;
 
   bool has_agg = !q.group_by.empty();
   for (auto& it : q.select) if (!it.is_star && contains_aggregate(*it.expr)) has_agg = true;
@@ -385,7 +488,7 @@ Plan bind_query(const Query& q, const std::string& table_name, const std::vector
       if (it.is_star) {
         if (!it.star_qualifier.empty() && it.star_qualifier != b.table)
           plan_error("Error during planning: Invalid qualifier " + it.star_qualifier);
-        for (size_t c = 0; c < fields.size(); ++c) {
+        for (size_t c = 0; c < plan.n_input_fields; ++c) {
           const Field& f = fields[c];
           if (f.type == DType::Null && f.format != "n") unsupported("column '" + f.name + "' has Arrow type '" + f.format + "'");
           OutputCol oc; oc.name = f.name;
@@ -537,6 +640,8 @@ Plan bind_query(const Query& q, const std::string& table_name, const std::vector
   }
   return plan;
 }
+
+}  // namespace
 
 Plan bind_join(const Query& q, const std::vector<std::string>& names, const std::vector<std::vector<Field>>& tables) {
   if (q.joins.size() != 1) {

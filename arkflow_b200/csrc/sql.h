@@ -43,6 +43,9 @@ struct Expr {
   // Func
   bool distinct = false;
   bool star_arg = false;  // count(*)
+  // Column: set by the planner on the node that replaced a json_* call — the index of its derived input column
+  // (Plan::derived); `name` then holds the call's display name.  -1 for columns of the input.
+  int derived = -1;
 
   ExprPtr clone() const;
 };

@@ -54,7 +54,7 @@ ExprPtr Expr::clone() const {
   auto e = std::make_unique<Expr>();
   e->kind = kind; e->name = name; e->qualifier = qualifier; e->lit_type = lit_type; e->i64 = i64;
   e->f64 = f64; e->b = b; e->str = str; e->op = op; e->cast_to = cast_to; e->negated = negated;
-  e->distinct = distinct; e->star_arg = star_arg;
+  e->distinct = distinct; e->star_arg = star_arg; e->derived = derived;
   for (auto& a : args) e->args.push_back(a->clone());
   return e;
 }

@@ -113,7 +113,11 @@ const char* ark_last_error(void); /* thread-local, valid until the next call on 
  * temporaries_resolved, evaluates the keys with ark_expr_evaluate and registers what Temporary::get
  * returns through ark_sql_process_tables.
  * NULL config → ARK_ERR_CONFIG ("Batch processor configuration is missing", sql.rs:235-239);
- * unparsable SQL → ARK_ERR_PROCESS ("SQL query error: …", sql.rs:92-98) at construction. */
+ * unparsable SQL → ARK_ERR_PROCESS ("SQL query error: …", sql.rs:92-98) at construction.
+ * The query may call the JSON path functions of datafusion-functions-json (registered by sql.rs:18-24):
+ * json_get_str / _int / _float / _bool / _json, json_as_text, json_contains, json_length on a Utf8 column or
+ * CAST(<Binary column> AS STRING) with up to 8 literal path elements (DESIGN.md §6.1).  The multi-table entry points
+ * and ark_expr_evaluate do not bind them (ARK_ERR_UNSUPPORTED, "scalar function …()"). */
 int ark_sql_create(const char* config_json, ark_proc_t** out);
 /* One RecordBatch (struct array + schema) in, one out.  Replaces SqlProcessor::process
  * (sql.rs:209-220) + execute_query (sql.rs:108-149). */
