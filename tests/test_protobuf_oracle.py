@@ -231,3 +231,119 @@ def test_oneof_keeps_the_last_member_on_the_wire():
         up = cls.FromString(payload)
         for f in fields:
             assert same(f.kind, dec[f.name], getattr(up, f.name)), (f.name, payload)
+
+
+# ---- the edges tests/test_protobuf_edges_gpu.py holds the library to ------------------------------------------------------
+def _key(num, wire):
+    out = bytearray()
+    put_varint(out, (num << 3) | wire)
+    return bytes(out)
+
+
+def _varint_form(v, length):
+    return bytes(((v >> (7 * i)) & 0x7F) | (0x80 if i < length - 1 else 0) for i in range(length))
+
+
+def _one(f, v):
+    return encode_message([PbField(f.name, f.number, f.kind, presence=True)], {f.name: v})
+
+
+def _same_message(fields, cls, payload):
+    dec = decode_message(fields, payload)
+    up = cls.FromString(payload)
+    for f in fields:
+        assert same(f.kind, dec[f.name], getattr(up, f.name)), (f.name, payload)
+
+
+FIELD_NUMBERS = [PbField(f"n{num}", num, kind) for num, kind in (
+    (2048, "sint64"), (1, "int32"), (15, "string"), (16, "fixed32"), (127, "bool"), (128, "double"), (129, "bytes"),
+    (2047, "uint64"), (262143, "float"), (262144, "enum"), (33554431, "sfixed64"), (33554432, "string"),
+    (536870911, "sint32"))]
+
+
+def test_large_field_numbers_and_skipped_groups_match_upb():
+    fields = FIELD_NUMBERS
+    cls = upb_class(fields)
+    rng = np.random.default_rng(31)
+    for _ in range(300):
+        values = {f.name: rand_value(rng, f.kind) for f in fields if rng.random() < 0.7}
+        for f in fields:  # A1
+            if f.kind in ("float", "double") and f.name in values and values[f.name] == 0.0:
+                values[f.name] = 0.0
+        got = encode_message(fields, values)
+        assert got == fill(cls, fields, values).SerializeToString(deterministic=True), values
+        # interleaved unknown neighbours and an unknown group holding known numbers with the wrong wire type
+        parts = [_one(f, rand_value(rng, f.kind)) for f in fields if rng.random() < 0.6]
+        parts += [_key(num, 0) + b"\x05" for num in (2, 130, 2049, 262145, 33554433, 536870910) if rng.random() < 0.5]
+        group = _key(130, 3) + _key(128, 0) + b"\x01" + _key(536870911, 1) + b"\x00" * 8 + _key(2048, 3) + _key(2048, 4) + _key(130, 4)
+        parts.append(group)
+        rng.shuffle(parts)
+        _same_message(fields, cls, b"".join(parts))
+
+
+def _wide(n):
+    groups = {31: 0, 32: 0, 40: 1, 41: 1, 42: 1, 62: 2, 63: 2}
+    return [PbField(f"w{j}", 65 - j if j % 3 != 2 else 300 + j, KINDS[j % len(KINDS)], oneof=groups.get(j)) for j in range(n)]
+
+
+def test_sixty_four_fields_and_oneofs_past_bit_32_match_upb():
+    fields = _wide(64)
+    cls = upb_class(fields)
+    rng = np.random.default_rng(64)
+    members = [fields[j] for j in (31, 32, 40, 41, 42, 62, 63)]
+    for _ in range(300):
+        parts = []
+        for _ in range(int(rng.integers(0, 8))):
+            f = members[int(rng.integers(0, len(members)))] if rng.random() < 0.6 else fields[int(rng.integers(0, 64))]
+            parts.append(_one(f, rand_value(rng, f.kind)))
+        _same_message(fields, cls, b"".join(parts))
+
+
+VARINT_KINDS = [PbField("i32", 1, "int32"), PbField("i64", 2, "int64"), PbField("u32", 3, "uint32"), PbField("u64", 4, "uint64"),
+                PbField("s32", 5, "sint32"), PbField("s64", 6, "sint64"), PbField("b", 7, "bool"), PbField("e", 8, "enum")]
+
+
+def test_overlong_and_out_of_range_varints_match_upb():
+    # overlong 0 / 1, the largest legal 10th byte, values past 2^32 for the 32-bit kinds (truncated; sint32 before the
+    # zigzag), 2 and 2^63 for bool; an overlong key
+    cls = upb_class(VARINT_KINDS)
+    forms = [(0, n) for n in range(1, 11)] + [(1, n) for n in range(1, 11)] + [
+        (2**64 - 1, 10), (2**63, 10), (2**32 + 2, 5), (2**32 + 5, 7), (2**33 - 1, 5), (0xFFFFFFFF80000000, 10), (2, 4),
+        (2**40 + 3, 10), (zigzag64(-2**40), 6)]
+    for f in VARINT_KINDS:
+        for v, n in forms:
+            _same_message(VARINT_KINDS, cls, _key(f.number, 0) + _varint_form(v, n))
+        _same_message(VARINT_KINDS, cls, _varint_form((f.number << 3), 3) + _varint_form(1, 2))
+    dec = decode_message(VARINT_KINDS, b"".join(_key(f.number, 0) + _varint_form(2**32 + 2, 5) for f in VARINT_KINDS))
+    assert (dec["i32"], dec["u32"], dec["s32"], dec["e"], dec["b"]) == (2, 2, 1, 2, True)
+    for f in VARINT_KINDS:  # 11 bytes: both reject it
+        with pytest.raises(ProtobufError):
+            decode_message(VARINT_KINDS, _key(f.number, 0) + b"\x80" * 10 + b"\x00")
+        with pytest.raises(Exception):
+            cls.FromString(_key(f.number, 0) + b"\x80" * 10 + b"\x00")
+
+
+UTF8_BAD = [b"\xc0\x80", b"\xc1\xbf", b"\xe0\x80\x80", b"\xe0\x9f\xbf", b"\xf0\x80\x80\x80", b"\xf0\x8f\xbf\xbf", b"\xed\xa0\x80",
+            b"\xed\xbf\xbf", b"\xf4\x90\x80\x80", b"\xf5\x80\x80\x80", b"\xff", b"\x80", b"a\xbfb", b"ab\xc3", b"ab\xe6\xbc",
+            b"ab\xf0\x9f\x98"]
+UTF8_GOOD = [b"\xc2\x80", b"\xdf\xbf", b"\xe0\xa0\x80", b"\xed\x9f\xbf", b"\xee\x80\x80", b"\xef\xbf\xbf", b"\xf0\x90\x80\x80",
+             b"\xf4\x8f\xbf\xbf", "ab😀".encode()]
+
+
+def test_utf8_forms_match_upb():
+    # proto3 `string`: upb checks UTF-8 as prost does; `bytes` takes anything
+    fields = [PbField("s", 1, "string"), PbField("b", 2, "bytes"), PbField("t", 3, "string")]
+    cls = upb_class(fields)
+    trap = _key(19, 0) + b"\x01"  # an unknown field whose key starts with a continuation byte
+    for x in UTF8_GOOD + UTF8_BAD:
+        as_bytes = _key(2, 2) + bytes([len(x)]) + x + trap
+        _same_message(fields, cls, as_bytes)
+        for payload in (_key(1, 2) + bytes([len(x)]) + x + trap, trap + _key(1, 2) + bytes([len(x)]) + x):
+            if x in UTF8_GOOD:
+                _same_message(fields, cls, payload)
+                continue
+            with pytest.raises(ProtobufError) as e:
+                decode_message(fields, payload)
+            assert "not UTF-8" in e.value.message
+            with pytest.raises(Exception):
+                cls.FromString(payload)
