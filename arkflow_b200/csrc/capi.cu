@@ -167,6 +167,7 @@ int ark_sql_partial_aggregate_device(ark_proc_t* p, ArrowDeviceArray* in, ArrowS
     if (n_parts < 1) fail(ARK_ERR_PROCESS, "n_parts must be >= 1");
     auto bound = sp->bind(in_schema);
     if (bound->plan->kind != Plan::Aggregate) fail(ARK_ERR_PROCESS, "partial aggregate requested for a query without aggregation");
+    refuse_limit_across_ranks(*bound->plan);
     StreamLease lease;
     Batch b = import_device(&view, in_schema, &bound->mask, in_owner, false, &bound->fields);
     if (!bound->plan->derived.empty()) b = append_json_columns(*bound->plan, b, lease.s);
@@ -187,6 +188,7 @@ int ark_sql_final_aggregate_device(ark_proc_t* p, ArrowDeviceArray* in, ArrowSch
     ArrowDeviceArray view = device_view(*in, in_owner);
     auto plan = sp->last_aggregate_plan();
     if (!plan) fail(ARK_ERR_PROCESS, "final aggregate called before any partial aggregate bound the query");
+    refuse_limit_across_ranks(*plan);
     StreamLease lease;
     Batch b = import_device(&view, in_schema, nullptr, in_owner);
     Batch r = run_final_aggregate(*plan, b, lease.s);

@@ -436,4 +436,45 @@ Batch run_filter_project(const Plan& plan, Batch& in, cudaStream_t stream) {
   return out;
 }
 
+void refuse_limit_across_ranks(const Plan& plan) {
+  if (plan.kind == Plan::Aggregate && plan.limit >= 0)
+    fail(ARK_ERR_UNSUPPORTED, "SQL outside the GPU subset: LIMIT on an aggregate split across ranks (each rank holds only part of the "
+                              "groups, so a per-rank LIMIT is not the query's LIMIT)");
+}
+
+// HAVING, computed items and LIMIT of an aggregate query: its stage plan over the group frame, on the call's stream.
+Batch run_group_stage(const Plan& plan, Batch& frame, cudaStream_t stream) {
+  if (!plan.stage) return frame;
+  const Plan& stage = *plan.stage;
+  if (frame.num_rows > 0) {
+    Batch r = run_filter_project(stage, frame, stream);
+    return stage.concats.empty() ? r : apply_concats(stage, r, stream);
+  }
+  // no group (a WHERE that kept no row): the filter kernels need a row, so the empty result is built here
+  Batch out;
+  out.input_name = frame.input_name;
+  BufferPtr z = device_alloc(16);
+  ARK_CUDA(cudaMemsetAsync(z.get(), 0, 16, stream));
+  auto empty = [&](const std::string& name, DType type, bool nullable) {
+    Column c;
+    c.field.name = name; c.field.type = type; c.field.nullable = nullable;
+    c.length = 0; c.data = (const uint8_t*)z.get(); c.data_bytes = 0;
+    if (type == DType::Utf8 || type == DType::Binary) { c.offsets = (const int32_t*)z.get(); c.first_offset = 0; }
+    c.owners = {z};
+    out.cols.push_back(c);
+  };
+  if (stage.concats.empty()) {
+    for (const OutputCol& oc : stage.outputs) empty(oc.name, oc.src.type, oc.src.nullable);
+  } else {
+    for (const FinalItem& fi : stage.final_items) {
+      if (!fi.is_concat) { const OutputCol& oc = stage.outputs[fi.index]; empty(oc.name, oc.src.type, oc.src.nullable); continue; }
+      const ConcatItem& ci = stage.concats[fi.index];
+      const bool cast_col = ci.is_cast && !ci.parts.empty() && !ci.parts[0].is_literal;
+      empty(ci.name, DType::Utf8, cast_col ? stage.outputs[ci.parts[0].out_index].src.nullable : true);
+    }
+  }
+  ARK_CUDA(cudaStreamSynchronize(stream));
+  return out;
+}
+
 }  // namespace ark

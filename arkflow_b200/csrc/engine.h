@@ -83,6 +83,10 @@ struct StagedColumn;  // decoded.h
 // meaning |raw| bytes of a string body whose escapes are decoded (json.cu).
 void launch_json_strings(const uint8_t* data, const StagedColumn& s, uint8_t* bytes, cudaStream_t stream);
 Batch run_aggregate(const Plan& plan, Batch& in, cudaStream_t stream);
+// The query's result from the group frame of an aggregate plan: the frame itself, or Plan::stage run over it.
+Batch run_group_stage(const Plan& plan, Batch& frame, cudaStream_t stream);
+// The multi-GPU aggregate entry points see part of the groups on each rank: an aggregate with LIMIT is refused there.
+void refuse_limit_across_ranks(const Plan& plan);
 Batch run_join(const Plan& plan, Batch& left, Batch& right, cudaStream_t stream);
 Batch run_partial_aggregate(const Plan& plan, Batch& in, int n_parts, std::vector<int64_t>& part_rows, cudaStream_t stream);
 Batch run_final_aggregate(const Plan& plan, Batch& partial, cudaStream_t stream);

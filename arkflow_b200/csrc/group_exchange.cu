@@ -361,6 +361,7 @@ int ark_sql_group_by_push_device(ark_proc_t* p, ark_dist_t* d, ArrowDeviceArray*
     if (c.pushed) fail(ARK_ERR_PROCESS, "ark_sql_group_by_push_device: the previous step has not been merged");
     auto bound = sp->bind(in_schema);
     if (bound->plan->kind != Plan::Aggregate) fail(ARK_ERR_PROCESS, "not an aggregate query");
+    refuse_limit_across_ranks(*bound->plan);
     StreamLease lease;
     Batch b = import_device(&view, in_schema, &bound->mask, in_owner, false, &bound->fields);
     if (!bound->plan->derived.empty()) b = append_json_columns(*bound->plan, b, lease.s);
@@ -380,6 +381,7 @@ int ark_sql_group_by_merge_device(ark_proc_t* p, ark_dist_t* d, ArrowDeviceArray
     if (!c.pushed) fail(ARK_ERR_PROCESS, "ark_sql_group_by_merge_device: nothing was pushed for this step");
     auto plan = sp->last_aggregate_plan();
     if (!plan) fail(ARK_ERR_PROCESS, "final aggregate before any partial aggregate");
+    refuse_limit_across_ranks(*plan);
     c.pushed = false;
     StreamLease lease;
     Batch r;

@@ -726,7 +726,7 @@ Batch run_aggregate(const Plan& plan, Batch& in, cudaStream_t stream) {
   Batch out = project_groups(plan, ex, outs, dg, key_src, stream, key_src2);
   ARK_CUDA(cudaStreamSynchronize(stream));
   return_table(plan, dg);
-  return out;
+  return run_group_stage(plan, out, stream);
 }
 
 // ---- multi-GPU building blocks (SURVEY.md §8(e)): partial states out, hash-partitioned; merge in ----
@@ -793,7 +793,7 @@ Batch run_final_aggregate(const Plan& plan, Batch& partial, cudaStream_t stream)
   Batch out = project_groups(plan, mx, outs, dg, key_cols ? &partial.cols[0] : nullptr, stream, key_cols == 2 ? &partial.cols[1] : nullptr);
   ARK_CUDA(cudaStreamSynchronize(stream));
   return_table(mp, dg);  // mp.hints is the plan's final_hints
-  return out;
+  return run_group_stage(plan, out, stream);
 }
 
 // ---- device-side exchange (group_exchange.cu): partial table → push over NVLink → merge → result --------------
@@ -941,6 +941,7 @@ bool run_group_by_merge(const Plan& plan, DistCtx& d, Batch& out, cudaStream_t s
   ARK_CUDA(cudaStreamSynchronize(stream));
   d.last_groups = G;
   return_table(hints, dg);
+  out = run_group_stage(plan, out, stream);
   return true;
 }
 

@@ -135,6 +135,10 @@ struct Plan {
   std::vector<std::string> key_names;
   std::vector<AggSpec> aggs;
   std::vector<PostItem> post;
+  // HAVING, computed SELECT items or LIMIT: `post` is the group frame (every key, then every distinct aggregate call of
+  // SELECT and HAVING) and this FilterProject plan over the frame yields the query's result (planner.cc, bind_stage).
+  // Null for every other aggregate query, whose result is `post` itself.
+  std::shared_ptr<const Plan> stage;
   std::shared_ptr<AggHints> hints = std::make_shared<AggHints>();
   std::shared_ptr<AggHints> final_hints = std::make_shared<AggHints>();  // table of the multi-GPU final merge
   // Join (two tables, inner equi-join)

@@ -345,6 +345,39 @@ void detect_simple_predicate(const Expr& w, const Binder& b, Plan& plan) {
   plan.simple = sp;
 }
 
+// One aggregate call: its function, argument and DataFusion name (sum(flow.value), count(*), avg for mean).
+AggSpec bind_aggregate(const Expr& e, const Binder& b) {
+  if (e.distinct) unsupported("aggregate DISTINCT");
+  AggSpec a;
+  std::string fn = e.name == "mean" ? "avg" : e.name;
+  if (fn == "count") {
+    if (e.star_arg || (e.args.size() == 1 && e.args[0]->kind == Expr::Literal && e.args[0]->lit_type != DType::Null)) {
+      a.func = AggFunc::CountStar;
+    } else {
+      if (e.args.size() != 1) plan_error("Error during planning: count expects one argument");
+      a.func = AggFunc::Count;
+      a.arg = b.value_source(*e.args[0]);
+    }
+    a.out_type = DType::Int64;
+  } else {
+    if (e.star_arg || e.args.size() != 1) plan_error("Error during planning: " + fn + " expects one argument");
+    if (contains_aggregate(*e.args[0])) plan_error("Error during planning: nested aggregates are not allowed");
+    a.arg = b.value_source(*e.args[0]);
+    if (!is_numeric(a.arg.type)) {
+      if ((fn == "min" || fn == "max")) unsupported(fn + " over " + dtype_name(a.arg.type));
+      plan_error("Error during planning: " + fn + " does not support " + dtype_name(a.arg.type));
+    }
+    if (fn == "sum") { a.func = AggFunc::Sum; a.out_type = a.arg.type; }
+    else if (fn == "avg") { a.func = AggFunc::Avg; a.out_type = DType::Float64; }
+    else if (fn == "min") { a.func = AggFunc::Min; a.out_type = a.arg.type; }
+    else { a.func = AggFunc::Max; a.out_type = a.arg.type; }
+  }
+  ExprPtr named = e.clone();
+  named->name = fn;
+  a.name = display(*named, b.table);
+  return a;
+}
+
 void bind_where(const Query& q, const Binder& b, Plan& plan) {
   if (!q.where) return;
   DType t = b.type_of(*q.where);
@@ -436,11 +469,120 @@ Query rewrite_json_calls(const Query& q, const Binder& b, Plan& plan) {
   }
   r.where = take(q.where);
   for (auto& g : q.group_by) r.group_by.push_back(take(g));
+  r.having = take(q.having);
   for (auto& o : q.order_by) r.order_by.push_back(take(o));
   return r;
 }
 
 Plan bind_single(const Query& q, Plan plan);
+
+// ---- HAVING, computed items and LIMIT of an aggregate query: a FilterProject stage over the group frame ----
+//
+// DataFusion plans these as Aggregate → Filter → Projection → Limit.  The aggregate here emits a *frame*: every GROUP BY
+// key, then every distinct aggregate call of SELECT and HAVING (plan.post / plan.aggs, hidden ones included).  SELECT
+// and HAVING are rewritten so that each key and each aggregate call reads a frame column, and the rewritten query
+// (WHERE = HAVING, the items, LIMIT) is bound by the single-table FilterProject binder into Plan::stage.  The frame's
+// columns are all "derived" columns of the stage plan: a Column node that reads one carries its display name, so the
+// stage's results are named as DataFusion names them (max(flow.value) - min(flow.value)).
+
+// The aggregate SELECT lists that bind without a stage: keys, aggregates, CAST(<aggregate> AS STRING) and literals.
+bool needs_stage(const Query& q) {
+  if (q.having || q.limit >= 0) return true;
+  for (auto& it : q.select) {
+    if (it.is_star) continue;
+    const Expr* e = it.expr.get();
+    if (e->kind == Expr::Cast && e->cast_to == DType::Utf8 && e->args[0]->kind == Expr::Func && is_aggregate_name(e->args[0]->name)) continue;
+    if ((e->kind == Expr::Func && is_aggregate_name(e->name)) || e->kind == Expr::Column || e->kind == Expr::Literal) continue;
+    return true;
+  }
+  return false;
+}
+
+struct FrameRewriter {
+  const Query& q;
+  const Binder& b;
+  const std::vector<std::string>& key_display;
+  Plan& plan;
+  std::vector<Field> fields;  // the frame's columns, in plan.post order
+
+  static ExprPtr frame_column(const std::vector<Field>& fields, int index) {
+    auto c = std::make_unique<Expr>();
+    c->kind = Expr::Column;
+    c->name = fields[index].name;
+    c->derived = index;
+    return c;
+  }
+
+  // Replaces every key and aggregate call under `e` by a frame column.  `clause` names the clause in the planning error
+  // of a column that is neither; in HAVING, an unqualified column named as a SELECT alias stands for that item's
+  // expression (datafusion-sql's resolve_aliases_to_exprs).
+  void rewrite(ExprPtr& e, const char* clause, bool aliases) {
+    if (e->kind == Expr::Func && is_aggregate_name(e->name)) {
+      for (auto& a : e->args)
+        if (contains_aggregate(*a)) plan_error("Error during planning: nested aggregates are not allowed");
+      AggSpec a = bind_aggregate(*e, b);
+      size_t k = 0;
+      while (k < plan.aggs.size() && plan.aggs[k].name != a.name) ++k;
+      if (k == plan.aggs.size()) {
+        const bool is_count = a.func == AggFunc::Count || a.func == AggFunc::CountStar;
+        PostItem pi;
+        pi.kind = PostItem::Agg; pi.index = (int)k; pi.name = a.name;
+        plan.post.push_back(pi);
+        fields.push_back(Field{a.name, a.out_type, !is_count, dtype_arrow_format(a.out_type)});
+        plan.aggs.push_back(std::move(a));
+      }
+      e = frame_column(fields, (int)(plan.keys.size() + k));
+      return;
+    }
+    if (e->kind == Expr::Column) {
+      if (aliases && e->qualifier.empty() && e->derived < 0)
+        for (auto& it : q.select)
+          if (!it.is_star && !it.alias.empty() && it.alias == e->name) {
+            e = it.expr->clone();
+            rewrite(e, clause, false);
+            return;
+          }
+      const std::string d = display(*e, b.table);
+      for (size_t k = 0; k < key_display.size(); ++k)
+        if (key_display[k] == d) { e = frame_column(fields, (int)k); return; }
+      b.resolve(*e);
+      plan_error(std::string("Error during planning: Column in ") + clause +
+                 " must be in GROUP BY or an aggregate function: While expanding wildcard, column \"" + e->name +
+                 "\" must appear in the GROUP BY clause or must be part of an aggregate function");
+    }
+    for (auto& a : e->args) rewrite(a, clause, aliases);
+  }
+};
+
+void bind_stage(const Query& q, const Binder& b, const std::vector<std::string>& key_display, Plan& plan) {
+  FrameRewriter fr{q, b, key_display, plan, {}};
+  for (size_t k = 0; k < plan.keys.size(); ++k) {
+    PostItem pi;
+    pi.kind = PostItem::Key; pi.index = (int)k; pi.name = key_display[k];
+    plan.post.push_back(pi);
+    fr.fields.push_back(Field{key_display[k], plan.keys[k].type, plan.keys[k].nullable, dtype_arrow_format(plan.keys[k].type)});
+  }
+  Query sq;
+  sq.from = q.from;
+  sq.limit = q.limit;
+  for (auto& it : q.select) {
+    if (it.is_star) plan_error("Error during planning: SELECT * is not valid with GROUP BY / aggregates");
+    SelectItem s;
+    s.expr = it.expr->clone();
+    s.alias = it.alias;
+    if (s.alias.empty() && s.expr->kind == Expr::Column) s.alias = s.expr->name;  // a bare key keeps its own name
+    fr.rewrite(s.expr, "SELECT", false);
+    sq.select.push_back(std::move(s));
+  }
+  if (q.having) {
+    sq.where = q.having->clone();
+    fr.rewrite(sq.where, "HAVING", true);
+  }
+  Plan stage;
+  stage.input_fields = fr.fields;
+  stage.n_input_fields = 0;  // every frame column is read through a derived Column node
+  plan.stage = std::make_shared<Plan>(bind_single(sq, std::move(stage)));
+}
 
 }  // namespace
 
@@ -472,8 +614,12 @@ Plan bind_single(const Query& q, Plan plan) {
 
   bool has_agg = !q.group_by.empty();
   for (auto& it : q.select) if (!it.is_star && contains_aggregate(*it.expr)) has_agg = true;
+  if (q.having && contains_aggregate(*q.having)) has_agg = true;
   if (q.where && contains_aggregate(*q.where))
     plan_error("Error during planning: Aggregate functions are not allowed in the WHERE clause");
+  if (q.having && !has_agg)
+    plan_error("Error during planning: HAVING clause references: " + display(*q.having, b.table) +
+               " must appear in the GROUP BY clause or be used in an aggregate function");
 
   bind_where(q, b, plan);
   // ORDER BY is accepted only where it cannot change the result: a global aggregate yields exactly one row
@@ -559,7 +705,6 @@ Plan bind_single(const Query& q, Plan plan) {
 
   // ---- aggregate ----
   plan.kind = Plan::Aggregate;
-  if (plan.limit >= 0) unsupported("LIMIT on an aggregate");
   std::vector<std::string> key_display;
   for (auto& g : q.group_by) {
     if (g->kind != Expr::Column) unsupported("GROUP BY on a computed expression");
@@ -571,6 +716,10 @@ Plan bind_single(const Query& q, Plan plan) {
     key_display.push_back(display(*g, b.table));
   }
   if (plan.keys.size() > 2) unsupported("more than two GROUP BY keys");
+  if (needs_stage(q)) {
+    bind_stage(q, b, key_display, plan);
+    return plan;
+  }
   for (auto& it : q.select) {
     if (it.is_star) plan_error("Error during planning: SELECT * is not valid with GROUP BY / aggregates");
     const Expr* ep = it.expr.get();
@@ -581,35 +730,7 @@ Plan bind_single(const Query& q, Plan plan) {
     }
     const Expr& e = *ep;
     if (e.kind == Expr::Func && is_aggregate_name(e.name)) {
-      if (e.distinct) unsupported("aggregate DISTINCT");
-      AggSpec a;
-      std::string fn = e.name == "mean" ? "avg" : e.name;
-      if (fn == "count") {
-        if (e.star_arg || (e.args.size() == 1 && e.args[0]->kind == Expr::Literal && e.args[0]->lit_type != DType::Null)) {
-          a.func = AggFunc::CountStar;
-        } else {
-          if (e.args.size() != 1) plan_error("Error during planning: count expects one argument");
-          a.func = AggFunc::Count;
-          if (e.args[0]->kind == Expr::Column) a.arg = b.value_source(*e.args[0]);
-          else a.arg = b.value_source(*e.args[0]);
-        }
-        a.out_type = DType::Int64;
-      } else {
-        if (e.star_arg || e.args.size() != 1) plan_error("Error during planning: " + fn + " expects one argument");
-        if (contains_aggregate(*e.args[0])) plan_error("Error during planning: nested aggregates are not allowed");
-        a.arg = b.value_source(*e.args[0]);
-        if (!is_numeric(a.arg.type)) {
-          if ((fn == "min" || fn == "max")) unsupported(fn + " over " + dtype_name(a.arg.type));
-          plan_error("Error during planning: " + fn + " does not support " + dtype_name(a.arg.type));
-        }
-        if (fn == "sum") { a.func = AggFunc::Sum; a.out_type = a.arg.type; }
-        else if (fn == "avg") { a.func = AggFunc::Avg; a.out_type = DType::Float64; }
-        else if (fn == "min") { a.func = AggFunc::Min; a.out_type = a.arg.type; }
-        else { a.func = AggFunc::Max; a.out_type = a.arg.type; }
-      }
-      ExprPtr named = e.clone();
-      named->name = fn;
-      a.name = display(*named, b.table);
+      AggSpec a = bind_aggregate(e, b);
       if (pi.cast_utf8 && a.out_type != DType::Int64) unsupported(std::string("CAST(") + dtype_name(a.out_type) + " aggregate AS STRING)");
       pi.kind = PostItem::Agg; pi.index = (int)plan.aggs.size();
       pi.name = it.alias.empty() ? a.name : it.alias;
@@ -654,6 +775,7 @@ Plan bind_join(const Query& q, const std::vector<std::string>& names, const std:
     unsupported("more than one JOIN");
   }
   if (q.where) unsupported("WHERE on a join query");
+  if (q.having) unsupported("HAVING on a join query");
   if (!q.group_by.empty()) unsupported("GROUP BY on a join query");
   if (q.limit >= 0) unsupported("LIMIT on a join query");
   auto find_table = [&](const std::string& n) -> int {

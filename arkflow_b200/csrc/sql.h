@@ -76,6 +76,7 @@ struct Query {
   std::vector<JoinClause> joins;
   ExprPtr where;
   std::vector<ExprPtr> group_by;
+  ExprPtr having;                 // aggregate queries only (plan.h: Plan::stage)
   std::vector<ExprPtr> order_by;  // accepted only where it cannot change the result (one-row global aggregates)
   int64_t limit = -1;
 };

@@ -259,7 +259,7 @@ struct Parser {
       expect_kw("BY");
       do { q.group_by.push_back(parse_expr()); } while (accept(Tok::Comma));
     }
-    if (is_kw("HAVING")) unsupported("HAVING");
+    if (accept_kw("HAVING")) q.having = parse_expr();
     if (accept_kw("ORDER")) {
       expect_kw("BY");
       do {

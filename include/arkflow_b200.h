@@ -117,7 +117,9 @@ const char* ark_last_error(void); /* thread-local, valid until the next call on 
  * The query may call the JSON path functions of datafusion-functions-json (registered by sql.rs:18-24):
  * json_get_str / _int / _float / _bool / _json, json_as_text, json_contains, json_length on a Utf8 column or
  * CAST(<Binary column> AS STRING) with up to 8 literal path elements (DESIGN.md §6.1).  The multi-table entry points
- * and ark_expr_evaluate do not bind them (ARK_ERR_UNSUPPORTED, "scalar function …()"). */
+ * and ark_expr_evaluate do not bind them (ARK_ERR_UNSUPPORTED, "scalar function …()").
+ * Aggregate queries may add HAVING, expressions over keys and aggregates in the SELECT list, and LIMIT (DESIGN.md §6);
+ * HAVING on a join query is ARK_ERR_UNSUPPORTED. */
 int ark_sql_create(const char* config_json, ark_proc_t** out);
 /* One RecordBatch (struct array + schema) in, one out.  Replaces SqlProcessor::process
  * (sql.rs:209-220) + execute_query (sql.rs:108-149). */
@@ -251,7 +253,9 @@ void ark_batch_destroy(ark_batcher_t* b);
 
 /* ---- multi-GPU GROUP BY / JOIN building blocks (device-resident; SURVEY.md §8(e)).  The
  *      exchange between them is the caller's NCCL all-to-all or the peer-memory pull below; nothing like this exists in the
- *      reference (DataFusion's RepartitionExec(Hash) is in-process). ---- */
+ *      reference (DataFusion's RepartitionExec(Hash) is in-process).  HAVING and computed items apply after the final
+ *      merge; an aggregate query with LIMIT is ARK_ERR_UNSUPPORTED on every aggregate entry point below and on the
+ *      ark_sql_group_by_* ones, since each rank holds only part of the groups. ---- */
 /* Partial aggregate of one local batch → (keys, partial states) batch, hash-partitioned into
  * n_parts contiguous row ranges; part_rows[n_parts] receives the row count of each range. */
 int ark_sql_partial_aggregate_device(ark_proc_t* p, struct ArrowDeviceArray* in,
